@@ -109,6 +109,11 @@ int occ_conv_bf16x3(const float* x, const float* w2, float* out, int B, int X, i
                     int KY, int KZ, int stride, int dil, const float* bias, const float* residual, int act,
                     int split_out, double* gn_stats, int cpg, void* workspace, size_t workspace_bytes,
                     occ_stream_t stream);
+/* The tiling occ_conv_bf16x3 uses for a conv shape ("same" padding): plan[0..3] = (tile rows 128 | 256, tile columns,
+ * ring stages, K splits).  splitk_ok = 0 answers for a conv with bias / residual / activation / split output or without a
+ * workspace (never split). */
+int occ_conv_plan(int B, int X, int Y, int Z, int Cin, int Cout, int KX, int KY, int KZ, int stride, int dil,
+                  int splitk_ok, int* plan);
 /* Several same-input stride-1 convolutions in ONE launch via an explicit tap table: taps = ntaps x (dx, dy, dz) input offsets
  * (HOST ints), w2 (Cout, ntaps*Cin) S32 tap-major in the table's order (zero where a branch does not use a tap).  The four
  * ASPP branches (1x1 + three dilated 3x3, P/occformer/backbones/modules/aspp.py:107-113) become one 25-tap launch. */

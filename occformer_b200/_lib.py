@@ -29,6 +29,7 @@ SIGNATURES = {
     "occ_gemm_bf16x3": (c_int, [P, P, P, c_int, c_int, c_int, P, P, c_int, c_int, P, c_int, c_int, STREAM]),
     "occ_conv_workspace_bytes": (c_size_t, []),
     "occ_conv_bf16x3": (c_int, [P, P, P] + [c_int] * 11 + [P, P, c_int, c_int, P, c_int, P, c_size_t, STREAM]),
+    "occ_conv_plan": (c_int, [c_int] * 12 + [P]),
     "occ_conv_taps_bf16x3": (c_int, [P, P, P] + [c_int] * 7 + [P, P, c_int, STREAM]),
     "occ_set_mma_passes": (c_int, [c_int]),
     "occ_get_mma_passes": (c_int, []),

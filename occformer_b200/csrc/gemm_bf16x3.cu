@@ -7,8 +7,8 @@
 // lo); each 32-k block is contracted by three bf16 tensor-core passes (hi*hi + lo*hi + hi*lo, fp32 accumulate): ~1e-5
 // relative error, the bytes, TMA boxes and shared-memory tiles of a plain fp32 operand.
 //
-// One CTA per SM, 288 threads: warp 8 = TMA producer (cp.async.bulk.tensor, 128B swizzle, STAGES-deep ring), warps 0-7 =
-// two consumer warpgroups.  Warpgroup g issues the wgmmas (bf16, M = 64, N = BN, K = 16, fp32 accumulators in registers)
+// One CTA per SM, 384 threads: warp 8 = TMA producer (cp.async.bulk.tensor, 128B swizzle, STAGES-deep ring; warps 9-11
+// only hand their registers to the consumers), warps 0-7 = two consumer warpgroups.  Warpgroup g issues the wgmmas (bf16, M = 64, N = BN, K = 16, fp32 accumulators in registers)
 // of rows 64g .. 64g+63 of the 128-row tile, then stages its accumulator in shared memory and runs the epilogue thread =
 // row (bias / activation / residual / GroupNorm statistics / pooling -> TMA store); the producer fills the ring for the
 // next tile meanwhile.  Conv mode never materialises im2col: every filter tap is a 5-D TMA box {32 ch, bz, by, bx, 1}
@@ -32,7 +32,8 @@ constexpr int EPI_BYTES = 8 /*warps*/ * EPI_BUF_BYTES;
 constexpr int CTRL_BYTES = 2048;   // mbarriers + fp64 GroupNorm partial sums of up to 96 groups; a multiple of 1024 so
                                    // that the swizzled epilogue staging buffers behind it stay 1024-byte aligned
 constexpr int MAX_STAT_GROUPS = 96;  // 2 * 96 doubles = 1536 B of CTRL_BYTES (barriers < 256 B)
-constexpr int GEMM_THREADS = 288;    // two consumer warpgroups + one producer warp
+constexpr int GEMM_THREADS = 384;    // two consumer warpgroups + one producer warpgroup (one TMA-issuing lane)
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;  // setmaxnreg: 128 * 40 + 256 * 232 <= 64 K registers
 constexpr int MAX_TAPS = 28;
 
 struct GemmParams {
@@ -121,21 +122,29 @@ constexpr int acc_pitch() { return BN + 8; }
 template <int BN>
 constexpr int acc_stage_bytes() { return 2 * 64 * acc_pitch<BN>() * 4; }
 
-template <int BN, int STAGES, bool LEAN>
+// MT = 2: a 256-row tile (two 128-row M tiles sharing every B k-block: a third fewer operand bytes per MAC at BN = 128).
+// Warpgroup cg runs two m64 chains over rows 128cg .. 128cg+127; chain h reads the 8-row atoms 16cg + 2i + h (SBO 2048),
+// so warp w of the warpgroup holds the 32 consecutive tile rows 128cg + 32w .. +31 (16 of each chain) and stages them
+// chunk by chunk through its own TMA-store buffer: no fp32 staging block, which leaves room for a 4-deep ring.
+// No pooling and no split-K.
+template <int BN, int STAGES, bool LEAN, int MT = 1>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
+                 const __grid_constant__ CUtensorMap tmC, const __grid_constant__ GemmParams p) {
   // LEAN = plain GEMM, whole 32-column chunks, TMA store, no conv addressing / pooling / GroupNorm statistics / split-K:
   // those branches compile away.
+  static_assert(MT == 1 || (MT == 2 && !LEAN), "paired M tiles: conv / full-epilogue instantiations only");
   const bool f_conv = !LEAN && p.conv != 0;
-  const bool f_pool = !LEAN && p.pool_out != nullptr;
+  const bool f_pool = !LEAN && MT == 1 && p.pool_out != nullptr;
   const bool f_stats = !LEAN && p.gn_stats != nullptr;
-  const int f_splits = LEAN ? 1 : p.splits;
+  const int f_splits = (LEAN || MT == 2) ? 1 : p.splits;
   const bool f_tma = LEAN || p.use_tma_store != 0;
   const bool f_store = LEAN || p.store_out != 0;
 
+  constexpr int TILE_M = MT * BM;
+  constexpr int A_BYTES = MT * A_STAGE_BYTES;
   constexpr int B_STAGE_BYTES = BN * BK * 4;
-  constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
+  constexpr int STAGE_BYTES = A_BYTES + B_STAGE_BYTES;
   constexpr int PITCH = acc_pitch<BN>();
 
   extern __shared__ uint8_t smem_raw[];
@@ -151,7 +160,7 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   const int lane = threadIdx.x & 31;
 
   const int num_n_tiles = (p.N + BN - 1) / BN;
-  const int num_m_tiles = f_conv ? p.B * p.tiles_x * p.tiles_y * p.tiles_z : (p.M + BM - 1) / BM;
+  const int num_m_tiles = f_conv ? p.B * p.tiles_x * p.tiles_y * p.tiles_z : (p.M + TILE_M - 1) / TILE_M;
   const int num_tiles = num_m_tiles * num_n_tiles * f_splits;
 
   if (warp == 8 && lane == 0) {
@@ -169,9 +178,10 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   }
   __syncthreads();
 
-  if (warp == 8) {
+  if (warp >= 8) {
     // ------------------------------------------------------------- TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == 8 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       const int cblocks = f_conv ? (p.Cin / BK) : 0;
@@ -203,7 +213,7 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * STAGE_BYTES;
-          uint8_t* sb = sa + A_STAGE_BYTES;
+          uint8_t* sb = sa + A_BYTES;
           mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
           if (f_conv) {
             // input offset of this tap: regular stencil (dilated, padding folded into c?0) or the explicit table
@@ -219,7 +229,7 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
               }
             }
           } else {
-            tma_load_2d(sa, &tmA, &full_bar[stage], kb * BK, m_tile * BM);
+            tma_load_2d(sa, &tmA, &full_bar[stage], kb * BK, m_tile * TILE_M);
           }
           tma_load_2d(sb, &tmB, &full_bar[stage], kb * BK, n_tile * BN);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -229,12 +239,13 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     }
   } else {
     // ------------------------------------------------------------- consumers: wgmma main loop + epilogue
+    setmaxnreg_inc<CONSUMER_REGS>();
     // warpgroup cg = warp >> 2 accumulates rows 64 cg .. 64 cg + 63 of the tile.  In the epilogue warp (cg, w) drains the
     // 32-row slab ew = 2 cg + (w & 1) for the chunks of parity wg = w >> 1 (the four warps of one parity cover the tile's
-    // 128 rows).
+    // 128 rows).  MT = 2: warp (cg, w) drains its own 32-row slab ew = 4 cg + w, every chunk.
     const int cg = warp >> 2;
-    const int ew = 2 * cg + (warp & 1);
-    const int wg = (warp >> 1) & 1;
+    const int ew = MT == 2 ? 4 * cg + (warp & 3) : 2 * cg + (warp & 1);
+    const int wg = MT == 2 ? 0 : (warp >> 1) & 1;
     const int et = ew * 32 + lane;   // thread index among the 128 threads of this chunk parity
     const int row = ew * 32 + lane;
     uint8_t* stage_buf = epi_smem + warp * EPI_BUF_BYTES;
@@ -253,22 +264,29 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
       const int n_tile = (tile / f_splits) % num_n_tiles;
       const int m_tile = tile / (f_splits * num_n_tiles);
       const int n0 = n_tile * BN;
+      float acc[MT][BN / 2];  // MT = 2: held in registers through the epilogue
       {
         const int split = tile % f_splits;
         const int kb0 = (int)(((long long)split * p.num_k_blocks) / f_splits);
         const int kb1 = (int)(((long long)(split + 1) * p.num_k_blocks) / f_splits);
-        float acc[BN / 2];
 #pragma unroll
-        for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+        for (int h = 0; h < MT; ++h)
+#pragma unroll
+          for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.f;
         int prev_stage = -1;
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&full_bar[stage], phase);
           const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-          const uint64_t adesc = make_sw128_desc(sa + cg * (64 * 128), 1024, 16);
-          const uint64_t bdesc = make_sw128_desc(sa + A_STAGE_BYTES, 1024, 16);
+          const uint64_t bdesc = make_sw128_desc(sa + A_BYTES, 1024, 16);
           wgmma_fence();
           // one S32 row block = 32 k values: hi*hi + lo*hi + hi*lo, six K=16 wgmmas stepping 32 bytes inside the row
-          wgmma_bf16x3_ss<BN>(acc, adesc, bdesc, 1u, p.passes);
+          if constexpr (MT == 1) {
+            wgmma_bf16x3_ss<BN>(acc[0], make_sw128_desc(sa + cg * (64 * 128), 1024, 16), bdesc, 1u, p.passes);
+          } else {
+            const uint32_t a0 = sa + cg * (128 * 128);
+            wgmma_bf16x3_ss2<BN>(acc[0], acc[MT - 1], make_sw128_desc(a0, 2048, 16), make_sw128_desc(a0 + 1024, 2048, 16),
+                                 bdesc, 1u, p.passes);
+          }
           wgmma_commit();
           wgmma_wait<1>();  // the previous k-block's wgmmas have finished reading their stage
           if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
@@ -276,18 +294,20 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
         wgmma_wait<0>();
-        wgmma_fence_regs(acc);
+#pragma unroll
+        for (int h = 0; h < MT; ++h) wgmma_fence_regs(acc[h]);
         if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-        // fragment -> row-major staging block of this warpgroup (the previous tile's epilogue finished reading it)
-        {
+        if constexpr (MT == 1) {
+          // fragment -> row-major staging block of this warpgroup (the previous tile's epilogue finished reading it)
           const int r0 = (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
           for (int j = 0; j < BN / 8; ++j) {
-            *reinterpret_cast<float2*>(acc_wg + r0 * PITCH + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
-            *reinterpret_cast<float2*>(acc_wg + (r0 + 8) * PITCH + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+            *reinterpret_cast<float2*>(acc_wg + r0 * PITCH + 8 * j + c0) = make_float2(acc[0][4 * j], acc[0][4 * j + 1]);
+            *reinterpret_cast<float2*>(acc_wg + (r0 + 8) * PITCH + 8 * j + c0) =
+                make_float2(acc[0][4 * j + 2], acc[0][4 * j + 3]);
           }
+          named_bar_sync(4 + cg, 128);
         }
-        named_bar_sync(4 + cg, 128);
       }
       // ---- output row of this thread
       long long m = -1;
@@ -306,9 +326,9 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         if (x < p.Xo && y < p.Yo && z < p.Zo)
           m = (((long long)tile_b * p.Xo + x) * p.Yo + y) * p.Zo + z;
       } else {
-        const long long mm = (long long)m_tile * BM + row;
+        const long long mm = (long long)m_tile * TILE_M + row;
         if (mm < p.M) m = mm;
-        if (p.rows_per_batch > 0) tile_b = (int)(((long long)m_tile * BM) / p.rows_per_batch);
+        if (p.rows_per_batch > 0) tile_b = (int)(((long long)m_tile * TILE_M) / p.rows_per_batch);
       }
       const bool valid = m >= 0;
       // pooled mode: this row's cell inside the tile and the (cell, column) slots this thread drains, once per tile
@@ -356,15 +376,45 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         }
         asm volatile("bar.sync 1, 256;" ::: "memory");
       }
-#pragma unroll 1
-      for (int c = wg; c < BN / 32; c += 2) {
+      constexpr int CHUNK_UNROLL = MT == 2 ? BN / 32 : 1;  // MT = 2 indexes the accumulator registers by chunk
+#pragma unroll CHUNK_UNROLL
+      for (int c = wg; c < BN / 32; c += 3 - MT) {
         const int nc = n0 + c * 32;
         if (nc >= p.N) break;
         float v[32];
+        if constexpr (MT == 1) {
 #pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          const float4 q = *reinterpret_cast<const float4*>(acc_row + c * 32 + j);
-          v[j] = q.x; v[j + 1] = q.y; v[j + 2] = q.z; v[j + 3] = q.w;
+          for (int j = 0; j < 32; j += 4) {
+            const float4 q = *reinterpret_cast<const float4*>(acc_row + c * 32 + j);
+            v[j] = q.x; v[j + 1] = q.y; v[j + 2] = q.z; v[j + 3] = q.w;
+          }
+        } else {
+          // the warp's fragment of chunk c -> its 128B-swizzled buffer, row = warp-local tile row (chain h, fragment
+          // row r: 8 h + r for r < 8, 16 + 8 h + r - 8 otherwise) -> v = row `lane`
+          if (lane == 0) tma_store_wait_read<0>();  // the previous chunk's TMA store has read the buffer
+          __syncwarp();
+          const int r = lane >> 2;
+#pragma unroll
+          for (int cc = 0; cc < BN / 32; ++cc) {
+            if (cc != c) continue;
+#pragma unroll
+            for (int h = 0; h < MT; ++h) {
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj) {
+                const int j = 4 * cc + jj, off = (((2 * jj + ((lane & 3) >> 1)) ^ r) << 4) + (lane & 1) * 8;
+                *reinterpret_cast<float2*>(stage_buf + (8 * h + r) * 128 + off) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
+                *reinterpret_cast<float2*>(stage_buf + (16 + 8 * h + r) * 128 + off) =
+                    make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
+              }
+            }
+          }
+          __syncwarp();
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const float4 q = *reinterpret_cast<const float4*>(stage_buf + lane * 128 + ((j ^ (lane & 7)) << 4));
+            v[4 * j] = q.x; v[4 * j + 1] = q.y; v[4 * j + 2] = q.z; v[4 * j + 3] = q.w;
+          }
+          __syncwarp();  // every lane has its row before the buffer takes the output chunk
         }
         if (f_stats) {
           // per-group sum / sumsq of the raw conv output, butterfly-reduced over the 32 rows of the warp
@@ -516,9 +566,9 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
                 tma_store_5d(&tmC, sb, nc, tile_z0 + r0 % p.bz, tile_y0 + (r0 / p.bz) % p.by,
                              tile_x0 + r0 / (p.bz * p.by), tile_b);
             } else if (f_splits > 1) {
-              tma_reduce_add_2d(&tmC, sb, nc, m_tile * BM + ew * 32);
+              tma_reduce_add_2d(&tmC, sb, nc, m_tile * TILE_M + ew * 32);
             } else {
-              tma_store_2d(&tmC, sb, nc, m_tile * BM + ew * 32);
+              tma_store_2d(&tmC, sb, nc, m_tile * TILE_M + ew * 32);
             }
             tma_store_commit();
           }
@@ -529,7 +579,7 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
             if (nc + j < p.N) orow[j] = v[j];
         }
       }
-      named_bar_sync(4 + cg, 128);  // the staging block of this warpgroup may be overwritten by the next tile
+      if constexpr (MT == 1) named_bar_sync(4 + cg, 128);  // the staging block may be overwritten by the next tile
       if (f_splits > 1) {  // publish: this split's reduce-adds are complete
         if (lane == 0) tma_store_wait_all();
         asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -607,26 +657,31 @@ conv_gn_stats_kernel(const float* __restrict__ out, double* __restrict__ stats, 
   if (threadIdx.x < 2 * groups) atomicAdd(&stats[(size_t)b * 2 * groups + threadIdx.x], sg[threadIdx.x]);
 }
 
-template <int BN, int STAGES, bool LEAN = false>
+// ring depth of an instantiation: as deep as the shared memory allows (MT = 2 has no fp32 staging block)
+constexpr int gemm_stages(int bn, int mt) { return mt == 2 ? 4 : bn <= 32 ? 8 : bn <= 64 ? 6 : bn <= 96 ? 4 : 3; }
+
+template <int BN, bool LEAN = false, int MT = 1>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmParams& p,
                        int num_tiles, cudaStream_t stream) {
-  constexpr size_t smem = (size_t)STAGES * (A_STAGE_BYTES + BN * BK * 4) + 1024 /*align*/ + CTRL_BYTES + EPI_BYTES +
-                          acc_stage_bytes<BN>();
+  constexpr int STAGES = gemm_stages(BN, MT);
+  constexpr size_t smem = (size_t)STAGES * (MT * A_STAGE_BYTES + BN * BK * 4) + 1024 /*align*/ + CTRL_BYTES + EPI_BYTES +
+                          (MT == 1 ? acc_stage_bytes<BN>() : 0);
   static_assert(smem <= 227 * 1024, "shared memory budget");
-  OCC_ENSURE_SMEM((gemm_bf16x3_kernel<BN, STAGES, LEAN>), smem);
+  OCC_ENSURE_SMEM((gemm_bf16x3_kernel<BN, STAGES, LEAN, MT>), smem);
   int grid = num_tiles < sm_count() ? num_tiles : sm_count();
   if (grid < 1) grid = 1;
-  gemm_bf16x3_kernel<BN, STAGES, LEAN><<<grid, GEMM_THREADS, smem, stream>>>(tmA, tmB, tmC, p);
+  gemm_bf16x3_kernel<BN, STAGES, LEAN, MT><<<grid, GEMM_THREADS, smem, stream>>>(tmA, tmB, tmC, p);
   OCC_LAUNCH_CHECK();
   return OCC_OK;
 }
 
 // N-tile: 96-wide tiles for the 192-channel neck / head matrices (N = 192, 576: no padded columns), else 32 / 64 / 128
-// (a consumer thread holds BN / 2 fp32 accumulators)
+// (a consumer thread holds BN / 2 fp32 accumulators per M chain)
 static int gemm_bn(int N) { return N <= 32 ? 32 : N <= 64 ? 64 : (N % 96 == 0 && N % 128 != 0) ? 96 : 128; }
 
+// mt = 2: 256-row tiles (conv mode, BN 96 / 128, no pooling, no split-K)
 static int dispatch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmC, const void* W, GemmParams& p, int num_m_tiles,
-                         cudaStream_t stream) {
+                         cudaStream_t stream, int mt = 1) {
   const int BN = gemm_bn(p.N);
   CUtensorMap tmB;
   uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.N};
@@ -636,6 +691,11 @@ static int dispatch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmC, const v
   if (rc) return rc;
   if (p.splits < 1) p.splits = 1;
   const int num_tiles = num_m_tiles * ((p.N + BN - 1) / BN) * p.splits;
+  if (mt == 2) {
+    OCC_REQUIRE(p.conv && p.splits == 1 && p.pool_out == nullptr && (BN == 96 || BN == 128));
+    if (BN == 96) return launch_gemm<96, false, 2>(tmA, tmB, tmC, p, num_tiles, stream);
+    return launch_gemm<128, false, 2>(tmA, tmB, tmC, p, num_tiles, stream);
+  }
   // plain Linear with whole 32-column chunks through the TMA store: the lean instantiation (shorter epilogue)
   const bool lean = !p.conv && p.splits == 1 && p.pool_out == nullptr && p.gn_stats == nullptr && p.use_tma_store &&
                     p.store_out && p.N % 32 == 0 && (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0 &&
@@ -643,17 +703,72 @@ static int dispatch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmC, const v
   if (lean) {
     switch (BN) {
       case 32: break;
-      case 64: return launch_gemm<64, 6, true>(tmA, tmB, tmC, p, num_tiles, stream);
-      case 96: return launch_gemm<96, 4, true>(tmA, tmB, tmC, p, num_tiles, stream);
-      default: return launch_gemm<128, 3, true>(tmA, tmB, tmC, p, num_tiles, stream);
+      case 64: return launch_gemm<64, true>(tmA, tmB, tmC, p, num_tiles, stream);
+      case 96: return launch_gemm<96, true>(tmA, tmB, tmC, p, num_tiles, stream);
+      default: return launch_gemm<128, true>(tmA, tmB, tmC, p, num_tiles, stream);
     }
   }
   switch (BN) {
-    case 32: return launch_gemm<32, 8>(tmA, tmB, tmC, p, num_tiles, stream);
-    case 64: return launch_gemm<64, 6>(tmA, tmB, tmC, p, num_tiles, stream);
-    case 96: return launch_gemm<96, 4>(tmA, tmB, tmC, p, num_tiles, stream);
-    default: return launch_gemm<128, 3>(tmA, tmB, tmC, p, num_tiles, stream);
+    case 32: return launch_gemm<32>(tmA, tmB, tmC, p, num_tiles, stream);
+    case 64: return launch_gemm<64>(tmA, tmB, tmC, p, num_tiles, stream);
+    case 96: return launch_gemm<96>(tmA, tmB, tmC, p, num_tiles, stream);
+    default: return launch_gemm<128>(tmA, tmB, tmC, p, num_tiles, stream);
   }
+}
+
+// Voxel box of a `rows`-row conv tile: power-of-two sides (so that every warp's 32-row slab is a sub-box for the TMA
+// store) with the fewest padded output voxels; ties keep the deepest z, then y extent.  E.g. 100 x 100 x 8 -> 4 x 4 x 8
+// (no padding) instead of 1 x 16 x 8 (12 % of the rows past the grid).
+static void conv_box(int Xo, int Yo, int Zo, int rows, int stride, int& bx, int& by, int& bz) {
+  auto padded = [](int n, int b) { return (long long)((n + b - 1) / b) * b; };
+  long long best = -1;
+  for (int z = rows; z >= 1; z >>= 1)
+    for (int y = rows / z; y >= 1; y >>= 1) {
+      const int x = rows / (z * y);
+      if (x * stride > 256 || y * stride > 256 || z * stride > 256) continue;
+      const long long v = padded(Xo, x) * padded(Yo, y) * padded(Zo, z);
+      if (best < 0 || v < best) { best = v; bx = x; by = y; bz = z; }
+    }
+}
+
+// Tiling of a regular-stencil conv (occ_conv_bf16x3): 256-row tiles (MT = 2) for long-K convs with N <= 128 per tile,
+// at least four waves of them and at most 5 % more padded rows than 128-row tiles, else 128-row tiles with split-K for the deep stages (few output tiles, long K = 27 *
+// Cin): a 512->512 conv on 50x50x4 voxels has 158 tiles for 132 SMs (second wave 20 % full), a 1024->1024 conv on 25x25x2
+// has 40.  Split-K needs `splitk_ok` (no bias / activation / residual / split output, TMA store, a workspace).
+struct ConvPlan { int mt, bn, stages, splits, bx, by, bz, tiles_x, tiles_y, tiles_z; };
+static ConvPlan conv_plan(int B, int Xo, int Yo, int Zo, int Cout, int stride, int num_k_blocks, bool splitk_ok) {
+  ConvPlan c{};
+  c.bn = gemm_bn(Cout);
+  const int n_tiles = (Cout + c.bn - 1) / c.bn;
+  const int sms = sm_count();
+  auto tile = [&](int rows) {  // -> number of M tiles
+    conv_box(Xo, Yo, Zo, rows, stride, c.bx, c.by, c.bz);
+    c.tiles_x = (Xo + c.bx - 1) / c.bx; c.tiles_y = (Yo + c.by - 1) / c.by; c.tiles_z = (Zo + c.bz - 1) / c.bz;
+    return (long long)B * c.tiles_x * c.tiles_y * c.tiles_z;
+  };
+  c.mt = 1;
+  c.splits = 1;
+  const long long m2 = tile(2 * BM), m1 = tile(BM);
+  if ((c.bn == 96 || c.bn == 128) && num_k_blocks >= 64 && m2 * n_tiles >= 4LL * sms && m2 * 2 * 100 <= m1 * 105) {
+    c.mt = 2;
+    tile(2 * BM);
+  } else {
+    const long long num_m_tiles = m1;
+    const long long tiles = num_m_tiles * n_tiles;
+    auto eff = [&](int s) { const long long t = tiles * s; return (double)t / (double)(((t + sms - 1) / sms) * sms); };
+    // (not below 8 M-tiles = 1024 output rows: such convs are latency-bound either way, and keeping them on the
+    // single-pass path keeps small problems bit-reproducible -- the reduce-add order of the splits is not fixed)
+    if (splitk_ok && num_m_tiles >= 8 && tiles < 2 * sms && num_k_blocks >= 64 && eff(1) < 0.85) {
+      int best = 1;
+      for (int sp = 2; sp <= 8 && sp * 8 <= num_k_blocks; ++sp) {
+        if (eff(sp) > eff(best) + 0.02) best = sp;
+        if (eff(best) >= 0.85) break;
+      }
+      c.splits = best;
+    }
+  }
+  c.stages = gemm_stages(c.bn, c.mt);
+  return c;
 }
 
 }  // namespace occ
@@ -721,18 +836,20 @@ extern "C" int occ_conv_bf16x3(const float* x, const float* w2, float* out, int 
   p.Xo = (X + 2 * p.padx - dil * (KX - 1) - 1) / stride + 1;
   p.Yo = (Y + 2 * p.pady - dil * (KY - 1) - 1) / stride + 1;
   p.Zo = (Z + 2 * p.padz - dil * (KZ - 1) - 1) / stride + 1;
-  p.bz = next_pow2(p.Zo) < BM ? next_pow2(p.Zo) : BM;
-  p.by = next_pow2(p.Yo) < BM / p.bz ? next_pow2(p.Yo) : BM / p.bz;
-  p.bx = BM / (p.bz * p.by);
-  p.tiles_x = (p.Xo + p.bx - 1) / p.bx;
-  p.tiles_y = (p.Yo + p.by - 1) / p.by;
-  p.tiles_z = (p.Zo + p.bz - 1) / p.bz;
   p.N = Cout; p.K = KX * KY * KZ * Cin; p.num_k_blocks = p.K / BK;
   p.M = B * p.Xo * p.Yo * p.Zo;
   p.out = out; p.ldo = Cout; p.bias = bias; p.residual = residual; p.ldr = Cout; p.act = act; p.split_out = split_out;
   p.gn_stats = gn_stats; p.cpg = cpg; p.rows_per_batch = 0;
   p.pool_out = nullptr; p.pool_flag = nullptr; p.store_out = 1;
-  OCC_REQUIRE(p.bx * stride <= 256 && p.by * stride <= 256 && p.bz * stride <= 256);
+  p.use_tma_store = (Cout % 4 == 0) && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+  // split-K: the raw conv output of the encoder has no bias / activation (GroupNorm follows), so the partial sums can
+  // meet in `out` through TMA reduce-add; the GroupNorm statistics are then taken from the finished tensor
+  const bool splitk_ok = p.use_tma_store && !bias && !residual && act == 0 && !split_out && workspace &&
+                         workspace_bytes >= SPLITK_SEMS * sizeof(int) && (reinterpret_cast<uintptr_t>(workspace) & 3) == 0;
+  const ConvPlan plan = conv_plan(B, p.Xo, p.Yo, p.Zo, Cout, stride, p.num_k_blocks, splitk_ok);
+  p.bx = plan.bx; p.by = plan.by; p.bz = plan.bz;
+  p.tiles_x = plan.tiles_x; p.tiles_y = plan.tiles_y; p.tiles_z = plan.tiles_z;
+  p.splits = plan.splits;
   CUtensorMap tmA;
   uint64_t dims[5] = {(uint64_t)Cin, (uint64_t)Z, (uint64_t)Y, (uint64_t)X, (uint64_t)B};
   uint64_t strides[4] = {(uint64_t)Cin * 4, (uint64_t)Z * Cin * 4, (uint64_t)Y * Z * Cin * 4,
@@ -742,7 +859,6 @@ extern "C" int occ_conv_bf16x3(const float* x, const float* w2, float* out, int 
   int rc = make_tmap_f32(&tmA, x, 5, dims, strides, box, estr);
   if (rc) return rc;
   CUtensorMap tmC = tmA;
-  p.use_tma_store = (Cout % 4 == 0) && (reinterpret_cast<uintptr_t>(out) & 15) == 0;
   if (p.use_tma_store) {
     // one epilogue warp owns 32 consecutive rows of the (bx, by, bz) box = a sub-box (ex, ey, ez)
     const int ez = p.bz < 32 ? p.bz : 32;
@@ -756,34 +872,12 @@ extern "C" int occ_conv_bf16x3(const float* x, const float* w2, float* out, int 
     if (rc) return rc;
   }
   const int num_m_tiles = B * p.tiles_x * p.tiles_y * p.tiles_z;
-  // Split-K for the deep stages (few output tiles, long K = 27 * Cin): a 512->512 conv on 50x50x4 voxels has 158 tiles
-  // for 132 SMs (second wave 20 % full), a 1024->1024 conv on 25x25x2 has 40.  The raw conv output of the encoder has
-  // no bias / activation (GroupNorm follows), so the partial sums can meet in `out` through TMA reduce-add; the
-  // GroupNorm statistics are then taken from the finished tensor.
-  p.splits = 1;
-  if (p.use_tma_store && !bias && !residual && act == 0 && !split_out && workspace &&
-      workspace_bytes >= SPLITK_SEMS * sizeof(int) && (reinterpret_cast<uintptr_t>(workspace) & 3) == 0) {
-    const int bn = gemm_bn(Cout);
-    const long long tiles = (long long)num_m_tiles * ((Cout + bn - 1) / bn);
-    const int sms = sm_count();
-    auto eff = [&](int s) { const long long t = tiles * s; return (double)t / (double)(((t + sms - 1) / sms) * sms); };
-    // (not below 8 M-tiles = 1024 output rows: such convs are latency-bound either way, and keeping them on the
-    // single-pass path keeps small problems bit-reproducible -- the reduce-add order of the splits is not fixed)
-    if (num_m_tiles >= 8 && tiles < 2 * sms && p.num_k_blocks >= 64 && eff(1) < 0.85) {
-      int best = 1;
-      for (int sp = 2; sp <= 8 && sp * 8 <= p.num_k_blocks; ++sp) {
-        if (eff(sp) > eff(best) + 0.02) best = sp;
-        if (eff(best) >= 0.85) break;
-      }
-      p.splits = best;
-    }
-  }
   if (p.splits > 1) {
     OCC_CUDA(cudaMemsetAsync(out, 0, (size_t)p.M * Cout * sizeof(float), stream));
     p.gn_stats = nullptr;
     p.splitk_sem = static_cast<int*>(workspace);
   }
-  rc = dispatch_gemm(tmA, tmC, w2, p, num_m_tiles, stream);
+  rc = dispatch_gemm(tmA, tmC, w2, p, num_m_tiles, stream, plan.mt);
   if (rc) return rc;
   if (p.splits > 1 && gn_stats) {
     const int rows_per_batch = p.Xo * p.Yo * p.Zo;
@@ -794,6 +888,18 @@ extern "C" int occ_conv_bf16x3(const float* x, const float* w2, float* out, int 
   return OCC_OK;
 }
 
+
+// The tiling occ_conv_bf16x3 picks for a conv shape (without a split-K workspace: splits = 1 for a conv that has a bias,
+// activation, residual or split output): plan[0..3] = (tile rows, tile columns, ring stages, K splits).
+extern "C" int occ_conv_plan(int B, int X, int Y, int Z, int Cin, int Cout, int KX, int KY, int KZ, int stride, int dil,
+                             int splitk_ok, int* plan) {
+  OCC_REQUIRE(plan && B > 0 && X > 0 && Y > 0 && Z > 0 && Cin > 0 && Cin % BK == 0 && Cout > 0);
+  OCC_REQUIRE((stride == 1 || stride == 2) && dil >= 1);
+  const int Xo = (X - 1) / stride + 1, Yo = (Y - 1) / stride + 1, Zo = (Z - 1) / stride + 1;  // "same" padding
+  const ConvPlan c = conv_plan(B, Xo, Yo, Zo, Cout, stride, KX * KY * KZ * Cin / BK, splitk_ok != 0);
+  plan[0] = c.mt * BM; plan[1] = c.bn; plan[2] = c.stages; plan[3] = c.splits;
+  return OCC_OK;
+}
 
 // Several same-input stride-1 convolutions in one launch: an explicit tap table instead of a regular stencil.
 // x (B,X,Y,Z,Cin) S32; taps: ntaps x (dx, dy, dz) input offsets (HOST ints, |offset| <= 127); w2 (Cout, ntaps*Cin) S32,
@@ -818,9 +924,7 @@ extern "C" int occ_conv_taps_bf16x3(const float* x, const float* w2, float* out,
     p.tdx[t] = (signed char)taps[3 * t]; p.tdy[t] = (signed char)taps[3 * t + 1]; p.tdz[t] = (signed char)taps[3 * t + 2];
   }
   p.B = B; p.Xo = X; p.Yo = Y; p.Zo = Z;
-  p.bz = next_pow2(Z) < BM ? next_pow2(Z) : BM;
-  p.by = next_pow2(Y) < BM / p.bz ? next_pow2(Y) : BM / p.bz;
-  p.bx = BM / (p.bz * p.by);
+  conv_box(X, Y, Z, BM, 1, p.bx, p.by, p.bz);
   p.tiles_x = (X + p.bx - 1) / p.bx; p.tiles_y = (Y + p.by - 1) / p.by; p.tiles_z = (Z + p.bz - 1) / p.bz;
   p.N = Cout; p.K = ntaps * Cin; p.num_k_blocks = p.K / BK; p.M = B * X * Y * Z;
   p.out = out; p.ldo = Cout; p.ldr = Cout; p.act = 0; p.split_out = 0;

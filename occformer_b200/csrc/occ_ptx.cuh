@@ -317,6 +317,24 @@ __device__ __forceinline__ void wgmma_bf16x3_ss(float (&d)[N / 2], uint64_t ades
   }
 }
 
+// The same for two M = 64 chains (two A tiles, two accumulators) on one B tile: the wgmmas of the two chains alternate,
+// so each chain's dependent wgmma overlaps with the other's; every chain keeps the accumulation order of the above.
+template <int N>
+__device__ __forceinline__ void wgmma_bf16x3_ss2(float (&d0)[N / 2], float (&d1)[N / 2], uint64_t adesc0, uint64_t adesc1,
+                                                 uint64_t bdesc, uint32_t acc0, int passes = 3) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    wgmma_ss<N>(d0, adesc0 + 2 * h, bdesc + 2 * h, h ? 1u : acc0);
+    wgmma_ss<N>(d1, adesc1 + 2 * h, bdesc + 2 * h, h ? 1u : acc0);
+    if (passes == 3) {
+      wgmma_ss<N>(d0, adesc0 + 2 * (2 + h), bdesc + 2 * h, 1u);
+      wgmma_ss<N>(d1, adesc1 + 2 * (2 + h), bdesc + 2 * h, 1u);
+      wgmma_ss<N>(d0, adesc0 + 2 * h, bdesc + 2 * (2 + h), 1u);
+      wgmma_ss<N>(d1, adesc1 + 2 * h, bdesc + 2 * (2 + h), 1u);
+    }
+  }
+}
+
 // Accumulator columns [16k, 16k + 16) of a 64-row fragment (wgmma_ss layout, values x[8k .. 8k+7]) -> the hi / lo register A
 // fragments of one K = 16 step of the next contraction (accumulator and A fragment share the row / column ownership).
 __device__ __forceinline__ void split_frag_k16(const float* x, uint32_t (&hi)[4], uint32_t (&lo)[4]) {
@@ -337,6 +355,13 @@ __device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t* bar) {
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// Per-thread register budget of the calling warpgroup (all four warps execute it): the producer warpgroup of a
+// warp-specialised kernel gives registers back, the consumer warpgroups take them.  N: multiple of 8 in [24, 256].
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");

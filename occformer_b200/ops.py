@@ -326,6 +326,14 @@ def conv(x_cl, w2, ksize, stride=1, dil=1, bias=None, residual=None, act=0, spli
     return out
 
 
+def conv_plan(B, X, Y, Z, Cin, Cout, ksize=(3, 3, 3), stride=1, dil=1, splitk_ok=True):
+    """The tiling conv() picks for this shape: (tile rows, tile columns, ring stages, K splits).  splitk_ok=False for a
+    conv with bias / residual / activation / split output (never split)."""
+    plan = (ctypes.c_int * 4)()
+    check(lib().occ_conv_plan(B, X, Y, Z, Cin, Cout, *ksize, stride, dil, int(splitk_ok), plan), "occ_conv_plan")
+    return tuple(plan)
+
+
 def conv_taps(x_cl, w2, taps, gn_stats=None, cpg=0):
     """Stride-1 convolution over an explicit tap table (several dilated branches in one launch): x_cl (B,X,Y,Z,Cin) S32,
     taps = [(dx, dy, dz), ...], w2 (Cout, len(taps)*Cin) S32 tap-major -> raw (B,X,Y,Z,Cout) fp32."""

@@ -1,5 +1,5 @@
 """Per-kernel timings at BASELINE sizes (CUDA events, L2 flushed between iterations).  Development aid;
-bench.py is the contract benchmark.  usage: python scripts/microbench.py [conv gemm attn tail neck lift]"""
+bench.py is the contract benchmark.  usage: python scripts/microbench.py [conv convs gemm attn tail neck lift]"""
 import json
 import os
 import sys
@@ -65,6 +65,35 @@ def main():
         res["conv3d_c192_bf16x3_ms"] = t
         res["conv3d_c192_alg_TFs"] = 2 * 27 * E * E * X * Y * Z / t / 1e9
         del x, xs, xc, xe
+    if "convs" in which:
+        # every 3x3x3 conv shape of one bench step (batch 4, nusc_200 grid, GroupNorm statistics as the pipeline asks
+        # for them), in three passes and in one: a one-pass time close to the three-pass time means the kernel is bound by
+        # operand bytes or latency, not by the tensor pipe.  Ceiling = H100 SXM data-sheet dense bf16 (989 TF/s) / 3.
+        Bc = 4
+        shapes = [  # name, Cin, Cout, input grid, stride, cpg
+            ("c128_s1_200x200x16", 128, 128, (200, 200, 16), 1, 4),
+            ("c192_s1_200x200x16", 192, 192, (200, 200, 16), 1, 2),
+            ("c128to256_s2_to100x100x8", 128, 256, (200, 200, 16), 2, 8),
+            ("c256_s1_100x100x8", 256, 256, (100, 100, 8), 1, 8),
+            ("c256to512_s2_to50x50x4", 256, 512, (100, 100, 8), 2, 16),
+            ("c512_s1_50x50x4", 512, 512, (50, 50, 4), 1, 16),
+            ("c512to1024_s2_to25x25x2", 512, 1024, (50, 50, 4), 2, 32),
+            ("c1024_s1_25x25x2", 1024, 1024, (25, 25, 2), 1, 32),
+        ]
+        for name, ci, co, (xi, yi, zi), s, cpg in shapes:
+            xs = ops.to_split(torch.randn(Bc, xi, yi, zi, ci, device=dev) * 0.5)
+            w2, ks = ops.repack_conv_weight(torch.randn(co, ci, 3, 3, 3) * 0.02)
+            w2 = w2.to(dev)
+            st = torch.zeros(Bc, co // cpg, 2, dtype=torch.float64, device=dev)
+            vout = Bc * ((xi - 1) // s + 1) * ((yi - 1) // s + 1) * ((zi - 1) // s + 1)
+            fl = 2.0 * 27 * ci * co * vout
+            for mode in ("fp32", "bf16"):
+                with ops.precision(mode):
+                    t = timeit(lambda: ops.conv(xs, w2, ks, stride=s, gn_stats=st, cpg=cpg), iters=5)
+                tfs = fl / t / 1e9
+                res[f"{name}_{mode}"] = {"ms": round(t, 3), "alg_TFs": round(tfs, 1),
+                                         "frac_of_3pass_ceiling": round(3 * tfs / 989.0, 3)}
+            del xs
     if "gemm" in which:
         a = ops.to_split(torch.randn(rows, C, device=dev))
         w = ops.split_weight(torch.randn(3 * C, C) * C ** -0.5).to(dev)
