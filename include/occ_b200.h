@@ -31,6 +31,9 @@ extern "C" {
 typedef struct CUstream_st* occ_stream_t; /* = cudaStream_t */
 
 int occ_version(void);
+/* Kernel launches and cudaMemsetAsync calls the library has enqueued in this process so far (host-side counter over
+ * all threads, devices and streams; a call captured into a CUDA graph counts once, at capture). */
+long long occ_launch_count(void);
 
 /* ---------------------------------------------------------------------------------------------------------
  * LSS voxel pooling.

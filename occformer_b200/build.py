@@ -24,7 +24,9 @@ def sources():
 
 
 def headers():
-    return sorted(f for f in os.listdir(CSRC) if f.endswith(".cuh") or f.endswith(".h"))
+    """paths of the headers every source may include: csrc's own and the C ABI header"""
+    return sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cuh") or f.endswith(".h")) + [
+        os.path.join(os.path.dirname(HERE), "include", "occ_b200.h")]
 
 
 def _mtime(p):
@@ -32,13 +34,13 @@ def _mtime(p):
 
 
 def needs_build():
-    newest = max(_mtime(os.path.join(CSRC, f)) for f in sources() + headers())
+    newest = max(_mtime(p) for p in [os.path.join(CSRC, f) for f in sources()] + headers())
     return _mtime(LIB) < newest
 
 
 def _compile(src):
     obj = os.path.join(CSRC, "build", src[:-3] + ".o")
-    hdr_m = max([_mtime(os.path.join(CSRC, h)) for h in headers()] + [0.0])
+    hdr_m = max([_mtime(h) for h in headers()] + [0.0])
     if _mtime(obj) >= max(_mtime(os.path.join(CSRC, src)), hdr_m):
         return obj, ""
     cmd = [NVCC] + FLAGS + ["-c", os.path.join(CSRC, src), "-o", obj]

@@ -1,9 +1,13 @@
-// Library-wide launch-time configuration (host side only; no device state).
+// Library-wide host state (no device state): the launch-time configuration and the launch counter.
+#include <atomic>
+
 #include "occ_common.cuh"
 
 namespace occ {
 static int g_mma_passes = 3;
+static std::atomic<long long> g_launches{0};
 int mma_passes() { return g_mma_passes; }
+void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 }  // namespace occ
 
 // passes = 3: every contraction is an fp32 problem in three bf16 tensor-core passes (default; the mode of every parity
@@ -17,3 +21,5 @@ extern "C" int occ_set_mma_passes(int passes) {
   return prev;
 }
 extern "C" int occ_get_mma_passes(void) { return occ::g_mma_passes; }
+
+extern "C" long long occ_launch_count(void) { return occ::g_launches.load(std::memory_order_relaxed); }

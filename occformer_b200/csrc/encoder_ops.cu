@@ -544,7 +544,7 @@ extern "C" int occ_aspp_gap_branch(const float* in, double* sums_ws, const float
   OCC_REQUIRE(in && sums_ws && wconv && gw && gb && cat);
   OCC_REQUIRE(B > 0 && rows_per_batch > 0 && ch % 32 == 0 && ch <= 1024 && groups > 0 && ch % groups == 0 && 256 % (ch / 4) == 0);
   OCC_REQUIRE(ldo % 32 == 0 && out_off % 32 == 0);  // the branch lands in the S32 concat buffer
-  OCC_CUDA(cudaMemsetAsync(sums_ws, 0, (size_t)B * ch * sizeof(double), stream));
+  OCC_MEMSET(sums_ws, 0, (size_t)B * ch * sizeof(double), stream);
   const int chunk = 256;
   dim3 grid((rows_per_batch + chunk - 1) / chunk, B);
   colsum_kernel<<<grid, 256, 0, stream>>>(in, sums_ws, rows_per_batch, ch, chunk);

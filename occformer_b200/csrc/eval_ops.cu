@@ -292,7 +292,7 @@ extern "C" int occ_panoptic_eval(const long long* x_sem, const long long* x_inst
   t.mask = (unsigned int)(cap - 1);
   t.shift = 64 - (63 - __builtin_clzll((unsigned long long)cap));
   const bool pan = parts & 2;
-  OCC_CUDA(cudaMemsetAsync(ws, 0, pan ? occ_panoptic_eval_workspace_bytes(n) : (size_t)PE_SC_WORDS * 8, stream));
+  OCC_MEMSET(ws, 0, pan ? occ_panoptic_eval_workspace_bytes(n) : (size_t)PE_SC_WORDS * 8, stream);
   long long blocks = (n + 255) / 256;
   if (blocks > (long long)sm_count() * 8) blocks = (long long)sm_count() * 8;
   pan_scan_kernel<<<(unsigned)blocks, 256, 0, stream>>>(x_sem, x_inst, y_sem, y_inst, n, K, ignore_mask, parts, t, sc);
@@ -314,7 +314,7 @@ extern "C" int occ_panoptic_eval(const long long* x_sem, const long long* x_inst
 extern "C" int occ_ssc_counts(const unsigned char* pred, const unsigned char* target, long long n, int K, int ignore,
                               long long* conf_ws, long long* out, cudaStream_t stream) {
   OCC_REQUIRE(pred && target && conf_ws && out && n >= 0 && K >= 2 && K <= EV_MAXK);
-  OCC_CUDA(cudaMemsetAsync(conf_ws, 0, (size_t)K * K * sizeof(long long), stream));
+  OCC_MEMSET(conf_ws, 0, (size_t)K * K * sizeof(long long), stream);
   if (n > 0) {
     long long blocks = (n + 256 * 16 - 1) / (256 * 16);
     const long long cap = (long long)sm_count() * 8;

@@ -777,7 +777,7 @@ extern "C" int occ_conv_bf16x3(const float* x, const float* w2, float* out, int 
   }
   const int num_m_tiles = B * p.tiles_x * p.tiles_y * p.tiles_z;
   if (p.splits > 1) {
-    OCC_CUDA(cudaMemsetAsync(out, 0, (size_t)p.M * Cout * sizeof(float), stream));
+    OCC_MEMSET(out, 0, (size_t)p.M * Cout * sizeof(float), stream);
     p.gn_stats = nullptr;
     p.splitk_sem = static_cast<int*>(workspace);
   }

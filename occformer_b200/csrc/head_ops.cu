@@ -808,7 +808,7 @@ extern "C" int occ_mask_pool(const float* mask, int* pooled, int* row_flag, int 
                              int Yo, int Zo, int Q, cudaStream_t stream) {
   OCC_REQUIRE(mask && pooled && row_flag && B > 0 && X > 0 && Y > 0 && Z > 0 && Xo > 0 && Yo > 0 && Zo > 0 && Q > 0);
   OCC_REQUIRE(Xo <= X && Yo <= Y && Zo <= Z);
-  OCC_CUDA(cudaMemsetAsync(row_flag, 0, (size_t)B * Q * sizeof(int), stream));
+  OCC_MEMSET(row_flag, 0, (size_t)B * Q * sizeof(int), stream);
   OCC_REQUIRE(Q <= 256 && (long long)B * Xo * Yo * Zo < (1ll << 31));
   OCC_REQUIRE(X < 32768 && Y < 32768 && Z < 32768);
   long long blocks = ((long long)B * Xo * Yo * Zo + 3) / 4;
@@ -905,7 +905,7 @@ extern "C" int occ_panoptic_voxels(const float* mask, int Qs, const float* cls, 
   OCC_REQUIRE((reinterpret_cast<uintptr_t>(mask) & 15) == 0 && (reinterpret_cast<uintptr_t>(table) & 15) == 0);
   const long long Vo = (long long)Xo * Yo * Zo;
   OCC_REQUIRE((Vo + 127) / 128 < (1ll << 31));
-  OCC_CUDA(cudaMemsetAsync(present, 0, (size_t)B * Qs * sizeof(int), stream));
+  OCC_MEMSET(present, 0, (size_t)B * Qs * sizeof(int), stream);
   panoptic_vox_argmax_kernel<<<dim3((unsigned)((Vo + 127) / 128), B), 128, 0, stream>>>(mask, Qs, Q, X, Y, Z, Xo, Yo, Zo,
                                                                                        qidx, present);
   OCC_LAUNCH_CHECK();
@@ -922,7 +922,7 @@ extern "C" int occ_panoptic_points(const float* mask, int Qs, const float* cls, 
   OCC_REQUIRE(Q > 0 && Q <= Qs && Qs <= PAN_MAXQ && Qs % 4 == 0 && NC >= 3 && NC - 1 <= 63);
   OCC_REQUIRE((reinterpret_cast<uintptr_t>(mask) & 15) == 0 && (reinterpret_cast<uintptr_t>(table) & 15) == 0);
   if (n == 0) return OCC_OK;
-  OCC_CUDA(cudaMemsetAsync(present, 0, (size_t)B * Qs * sizeof(int), stream));
+  OCC_MEMSET(present, 0, (size_t)B * Qs * sizeof(int), stream);
   panoptic_pts_argmax_kernel<<<dim3((n + 127) / 128, B), 128, 0, stream>>>(
       mask, Qs, Q, X, Y, Z, pts, pts_stride, n, x_min, y_min, z_min, x_max - x_min, y_max - y_min, z_max - z_min, border,
       qidx, present);

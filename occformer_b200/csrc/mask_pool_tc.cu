@@ -234,8 +234,8 @@ extern "C" int occ_mask_gemm_pool(const float* mf, const float* membed, int* poo
   else if (w == 4 && X % 4 == 0 && Y % 4 == 0 && Z % 8 == 0) launch = launch_mask_pool<4, 4, 4, 8>;
   else if (w == 8 && X % 8 == 0 && Y % 8 == 0 && Z % 8 == 0) launch = launch_mask_pool<8, 8, 2, 8>;
   else return OCC_EUNSUPPORTED;
-  OCC_CUDA(cudaMemsetAsync(flag, 0, (size_t)B * Q * sizeof(int), stream));
+  OCC_MEMSET(flag, 0, (size_t)B * Q * sizeof(int), stream);
   // w = 8: a box holds a quarter of a cell, the partial maxima meet through atomicMax on the ordered ints
-  if (w == 8) OCC_CUDA(cudaMemsetAsync(pooled, 0x80, (size_t)B * Xo * Yo * Zo * Q * sizeof(int), stream));
+  if (w == 8) OCC_MEMSET(pooled, 0x80, (size_t)B * Xo * Yo * Zo * Q * sizeof(int), stream);
   return launch(mf, p, B, X, Y, Z, stream);
 }

@@ -7,6 +7,8 @@
 
 #include <type_traits>
 
+#include "../../include/occ_b200.h"  // every extern "C" definition is compiled against its declaration
+
 // C-ABI return convention (include/occ_b200.h): 0 = ok, negative = argument error,
 // positive = cudaError_t of the failed runtime call / launch.
 #define OCC_OK 0
@@ -28,13 +30,25 @@
     if (e__ != cudaSuccess) return static_cast<int>(e__); \
   } while (0)
 
+// Follows every kernel launch (exactly one per executed launch): returns the launch error, else counts the launch.
 #define OCC_LAUNCH_CHECK()                              \
   do {                                                  \
     cudaError_t e__ = cudaGetLastError();               \
     if (e__ != cudaSuccess) return static_cast<int>(e__); \
+    occ::count_launch();                                \
+  } while (0)
+
+// cudaMemsetAsync, checked and counted like a launch
+#define OCC_MEMSET(ptr, value, bytes, stream)                          \
+  do {                                                                 \
+    OCC_CUDA(cudaMemsetAsync((ptr), (value), (bytes), (stream)));      \
+    occ::count_launch();                                               \
   } while (0)
 
 namespace occ {
+
+// Adds one to the process-wide count of enqueued launches and memsets (occ_launch_count, csrc/config.cu).
+void count_launch();
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,

@@ -338,7 +338,7 @@ extern "C" int occ_lift_splat(const float* depth_prob, const float* feat_cl, con
   VpWorkspace ws;
   OCC_REQUIRE(vp_layout(workspace, P, V, &ws) <= workspace_bytes);
   // head[V] and counts[V] are adjacent in the workspace: one memset
-  OCC_CUDA(cudaMemsetAsync(ws.head, 0, reinterpret_cast<char*>(ws.counts + V) - reinterpret_cast<char*>(ws.head), stream));
+  OCC_MEMSET(ws.head, 0, reinterpret_cast<char*>(ws.counts + V) - reinterpret_cast<char*>(ws.head), stream);
   const VpGrid vg{dx0, dx1, dx2, bx0, bx1, bx2, nx0, nx1, nx2, X, Y, Z};
   vp_index_geom_kernel<<<(P + 255) / 256, 256, 0, stream>>>(geom, P, N * D * HW, vg, ws.vox_id, ws.counts, ws.head, ws.next);
   OCC_LAUNCH_CHECK();
@@ -361,7 +361,7 @@ extern "C" int occ_bev_pool(const float* feats, const long long* coords, float* 
   const int V = (int)Vll;
   VpWorkspace ws;
   OCC_REQUIRE(vp_layout(workspace, n, V, &ws) <= workspace_bytes);
-  OCC_CUDA(cudaMemsetAsync(ws.head, 0, reinterpret_cast<char*>(ws.counts + V) - reinterpret_cast<char*>(ws.head), stream));
+  OCC_MEMSET(ws.head, 0, reinterpret_cast<char*>(ws.counts + V) - reinterpret_cast<char*>(ws.head), stream);
   if (n > 0) {
     vp_index_coords_kernel<<<(n + 255) / 256, 256, 0, stream>>>(coords, n, B, X, Y, Z, ws.vox_id, ws.counts, ws.head,
                                                                 ws.next);
@@ -411,7 +411,7 @@ extern "C" int occ_voxel_pool_geom(const float* feats, const float* geom, float*
   const int P = (int)Pll, V = (int)Vll;
   VpWorkspace ws;
   OCC_REQUIRE(vp_layout(workspace, P, V, &ws) <= workspace_bytes);
-  OCC_CUDA(cudaMemsetAsync(ws.head, 0, reinterpret_cast<char*>(ws.counts + V) - reinterpret_cast<char*>(ws.head), stream));
+  OCC_MEMSET(ws.head, 0, reinterpret_cast<char*>(ws.counts + V) - reinterpret_cast<char*>(ws.head), stream);
   const VpGrid vg{dx0, dx1, dx2, bx0, bx1, bx2, nx0, nx1, nx2, X, Y, Z};
   vp_index_geom_kernel<<<(P + 255) / 256, 256, 0, stream>>>(geom, P, points_per_batch, vg, ws.vox_id, ws.counts, ws.head,
                                                              ws.next);
@@ -642,7 +642,7 @@ extern "C" int occ_lift_splat_fused(const float* depth_logits, long long logits_
   const int P = (int)Pll, V = (int)Vll;
   VpWorkspace ws;
   OCC_REQUIRE(vp_layout(workspace, P, V, &ws) <= workspace_bytes);
-  OCC_CUDA(cudaMemsetAsync(ws.head, 0, reinterpret_cast<char*>(ws.counts + V) - reinterpret_cast<char*>(ws.head), stream));
+  OCC_MEMSET(ws.head, 0, reinterpret_cast<char*>(ws.counts + V) - reinterpret_cast<char*>(ws.head), stream);
   const VpGrid vg{dx0, dx1, dx2, bx0, bx1, bx2, nx0, nx1, nx2, X, Y, Z};
   const int tiles_p = (HW + 31) / 32, tiles_c = (C + 31) / 32;
   const int nb_front = B * N * tiles_p;

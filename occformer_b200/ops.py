@@ -9,16 +9,29 @@ import torch
 
 from ._lib import check, lib
 
-LAUNCH_COUNT = [0]  # kernels launched by this library (bench.py reports it as gpu_launches)
+
+class _LaunchCount:
+    """``LAUNCH_COUNT[0]``: kernel launches and memsets the library has enqueued in this process (occ_launch_count;
+    bench.py reports it as gpu_launches)."""
+
+    def __getitem__(self, i):
+        if i != 0:
+            raise IndexError(i)
+        return lib().occ_launch_count()
 
 
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else ctypes.c_void_p(0)
+LAUNCH_COUNT = _LaunchCount()
 
 
-def _stream(t=None):
-    """the current torch stream of the tensor's device (tensors of one call share a device, checked by _chk)"""
-    return ctypes.c_void_p(torch.cuda.current_stream(t.device if t is not None else None).cuda_stream)
+def _stream():
+    """the current torch stream of the current device (where _chk requires a call's tensors to live)"""
+    return torch.cuda.current_stream().cuda_stream
+
+
+def _call(name, *args):
+    """lib().<name>(*args, current stream) with tensors passed as device pointers and None as NULL; raises RuntimeError
+    on a non-zero return code."""
+    check(getattr(lib(), name)(*(a.data_ptr() if torch.is_tensor(a) else a for a in args), _stream()), name)
 
 
 def _chk(t, name, dtype=torch.float32):
@@ -87,8 +100,7 @@ def to_split(x):
     _chk(x, "x")
     C = x.shape[-1]
     out = torch.empty_like(x)
-    check(lib().occ_split_rows(_ptr(x), _ptr(out), x.numel() // C, C, _stream(x)), "occ_split_rows")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_split_rows", x, out, x.numel() // C, C)
     return out
 
 
@@ -96,8 +108,7 @@ def from_split(x):
     _chk(x, "x")
     C = x.shape[-1]
     out = torch.empty_like(x)
-    check(lib().occ_unsplit_rows(_ptr(x), _ptr(out), x.numel() // C, C, _stream(x)), "occ_unsplit_rows")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_unsplit_rows", x, out, x.numel() // C, C)
     return out
 
 
@@ -170,9 +181,7 @@ def lss_geometry(frustum, rots, trans, intrins, post_rots, post_trans, bda):
     f = lambda t: _chk(t.float().contiguous(), "camera matrix")  # noqa: E731
     geom = torch.empty((B, N, D, fH, fW, 3), dtype=torch.float32, device=frustum.device)
     fr, r, t, k, pr, pt, bd = f(frustum), f(rots), f(trans), f(intrins), f(post_rots), f(post_trans), f(bda)
-    check(lib().occ_lss_geometry(_ptr(fr), D * fH * fW, _ptr(r), _ptr(t), _ptr(k), k.shape[-2], k.shape[-1], _ptr(pr),
-                                 _ptr(pt), _ptr(bd), bd.shape[-1], B, N, _ptr(geom), _stream(geom)), "occ_lss_geometry")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_lss_geometry", fr, D * fH * fW, r, t, k, k.shape[-2], k.shape[-1], pr, pt, bd, bd.shape[-1], B, N, geom)
     return geom
 
 
@@ -183,9 +192,7 @@ def lift_prologue(depth_logits, img_feat):
     C = img_feat.shape[1]
     prob = torch.empty_like(depth_logits)
     feat_cl = torch.empty((BN, fH * fW, C), dtype=torch.float32, device=img_feat.device)
-    check(lib().occ_lift_prologue(_ptr(depth_logits), _ptr(img_feat), _ptr(prob), _ptr(feat_cl), BN, D, C, fH * fW,
-                                  _stream()), "occ_lift_prologue")
-    LAUNCH_COUNT[0] += 2
+    _call("occ_lift_prologue", depth_logits, img_feat, prob, feat_cl, BN, D, C, fH * fW)
     return prob, feat_cl
 
 
@@ -201,9 +208,7 @@ def lift_splat(depth_prob, feat_cl, geom, B, N, dx, bx, nx, grid, return_workspa
     out = torch.empty((B, X, Y, Z, C), dtype=torch.float32, device=geom.device)
     out_s = torch.empty_like(out) if with_split else None
     f = [float(v) for v in (*dx, *bx, *nx)]
-    check(lib().occ_lift_splat(_ptr(depth_prob), _ptr(feat_cl), _ptr(geom), _ptr(out), _ptr(out_s), B, N, D, fH * fW, C,
-                               *f, X, Y, Z, _ptr(ws.buf), ws.nbytes, _stream(geom)), "occ_lift_splat")
-    LAUNCH_COUNT[0] += 3
+    _call("occ_lift_splat", depth_prob, feat_cl, geom, out, out_s, B, N, D, fH * fW, C, *f, X, Y, Z, ws.buf, ws.nbytes)
     res = (out, out_s) if with_split else out
     return (res, ws) if return_workspace else res
 
@@ -236,11 +241,8 @@ def lift_splat_fused(depth_logits, img_feat, frustum, rots, trans, intrins, post
     out = torch.empty((B, X, Y, Z, C), dtype=torch.float32, device=dev)
     out_s = torch.empty_like(out) if with_split else None
     fl = [float(v) for v in (*dx, *bx, *nx)]
-    check(lib().occ_lift_splat_fused(_ptr(depth_logits), ls, _ptr(img_feat), fs, _ptr(fr), _ptr(r), _ptr(t), _ptr(k), k.shape[-2],
-                                     k.shape[-1], _ptr(pr), _ptr(pt), _ptr(bd), bd.shape[-1], _ptr(prob), _ptr(feat_cl),
-                                     _ptr(out), _ptr(out_s), B, N, D, HW, C, *fl, X, Y, Z, _ptr(ws.buf), ws.nbytes,
-                                     _stream(prob)), "occ_lift_splat_fused")
-    LAUNCH_COUNT[0] += 3
+    _call("occ_lift_splat_fused", depth_logits, ls, img_feat, fs, fr, r, t, k, k.shape[-2], k.shape[-1], pr, pt, bd,
+          bd.shape[-1], prob, feat_cl, out, out_s, B, N, D, HW, C, *fl, X, Y, Z, ws.buf, ws.nbytes)
     return ((out, out_s) if with_split else out), prob
 
 
@@ -252,9 +254,7 @@ def voxel_pool_geom(feats, geom, B, dx, bx, nx, grid, return_workspace=False):
     ws = _workspace(P_, B, X, Y, Z, feats.device)
     out = torch.empty((B, X, Y, Z, C), dtype=torch.float32, device=feats.device)
     f = [float(v) for v in (*dx, *bx, *nx)]
-    check(lib().occ_voxel_pool_geom(_ptr(feats), _ptr(geom), _ptr(out), B, P_ // B, C, *f, X, Y, Z, _ptr(ws.buf),
-                                    ws.nbytes, _stream()), "occ_voxel_pool_geom")
-    LAUNCH_COUNT[0] += 3
+    _call("occ_voxel_pool_geom", feats, geom, out, B, P_ // B, C, *f, X, Y, Z, ws.buf, ws.nbytes)
     return (out, ws) if return_workspace else out
 
 
@@ -263,9 +263,7 @@ def bev_pool_channel_last(feats, coords, B, X, Y, Z, return_workspace=False):
     n, C = feats.shape
     ws = _workspace(n, B, X, Y, Z, feats.device)
     out = torch.empty((B, X, Y, Z, C), dtype=torch.float32, device=feats.device)
-    check(lib().occ_bev_pool(_ptr(feats), _ptr(coords), _ptr(out), n, C, B, X, Y, Z, _ptr(ws.buf), ws.nbytes,
-                             _stream()), "occ_bev_pool")
-    LAUNCH_COUNT[0] += 3
+    _call("occ_bev_pool", feats, coords, out, n, C, B, X, Y, Z, ws.buf, ws.nbytes)
     return (out, ws) if return_workspace else out
 
 
@@ -286,9 +284,7 @@ def gemm(a, w, bias=None, residual=None, act=0, split_out=False, out=None):
     if residual is not None:
         _chk(residual, "residual")
         assert residual.shape == (M, N)
-    check(lib().occ_gemm_bf16x3(_ptr(a), _ptr(w), _ptr(out), M, N, K, _ptr(bias), _ptr(residual), act, int(split_out),
-                                _stream(a)), "occ_gemm_bf16x3")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_gemm_bf16x3", a, w, out, M, N, K, bias, residual, act, int(split_out))
     return out
 
 
@@ -320,10 +316,8 @@ def conv(x_cl, w2, ksize, stride=1, dil=1, bias=None, residual=None, act=0, spli
     if gn_stats is not None:
         _chk(gn_stats, "gn_stats", torch.float64)
     ws = _conv_workspace(x_cl.device)
-    check(lib().occ_conv_bf16x3(_ptr(x_cl), _ptr(w2), _ptr(out), B, X, Y, Z, Cin, Cout, KX, KY, KZ, stride, dil,
-                                _ptr(bias), _ptr(residual), act, int(split_out), _ptr(gn_stats), cpg, _ptr(ws),
-                                ws.numel(), _stream(x_cl)), "occ_conv_bf16x3")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_conv_bf16x3", x_cl, w2, out, B, X, Y, Z, Cin, Cout, KX, KY, KZ, stride, dil, bias, residual, act,
+          int(split_out), gn_stats, cpg, ws, ws.numel())
     return out
 
 
@@ -347,9 +341,7 @@ def conv_taps(x_cl, w2, taps, gn_stats=None, cpg=0):
     arr = (ctypes.c_int * len(flat))(*flat)
     if gn_stats is not None:
         _chk(gn_stats, "gn_stats", torch.float64)
-    check(lib().occ_conv_taps_bf16x3(_ptr(x_cl), _ptr(w2), _ptr(out), B, X, Y, Z, Cin, Cout, len(taps), arr, _ptr(gn_stats),
-                                     cpg, _stream(x_cl)), "occ_conv_taps_bf16x3")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_conv_taps_bf16x3", x_cl, w2, out, B, X, Y, Z, Cin, Cout, len(taps), arr, gn_stats, cpg)
     return out
 
 
@@ -409,9 +401,7 @@ def gn_relu_zmean_ln(y, stats, gn_w, gn_b, ln_w, ln_b, B, XY, Z, C, groups, X=0,
         assert X > 0 and XY % X == 0
         tokn = window_layout_buffer(B, X, XY // X, Z, C, win_shift, y.device)
         ws = int(bool(win_shift))
-    check(lib().occ_gn_relu_zmean_ln(_ptr(y), _ptr(stats), _ptr(gn_w), _ptr(gn_b), _ptr(ln_w), _ptr(ln_b), _ptr(tok),
-                                     _ptr(tokn), B, XY, Z, C, groups, X, ws, _stream()), "occ_gn_relu_zmean_ln")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_gn_relu_zmean_ln", y, stats, gn_w, gn_b, ln_w, ln_b, tok, tokn, B, XY, Z, C, groups, X, ws)
     return tok, tokn
 
 
@@ -419,8 +409,7 @@ def layernorm(x, w, b, split_out=False):
     _chk(x, "x")
     rows, C = x.shape
     out = torch.empty_like(x)
-    check(lib().occ_layernorm(_ptr(x), _ptr(w), _ptr(b), _ptr(out), rows, C, int(split_out), _stream(x)), "occ_layernorm")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_layernorm", x, w, b, out, rows, C, int(split_out))
     return out
 
 
@@ -430,9 +419,7 @@ def swin_proj_ffn(att, tok, wp, bp, ln_w, ln_b, w1, b1, w2, b2):
     M, C = att.shape
     assert tok.shape == (M, C) and wp.shape == (C, C) and w1.shape == (C, C) and w2.shape == (C, C)
     out = torch.empty_like(att)
-    check(lib().occ_swin_proj_ffn(_ptr(att), _ptr(tok), _ptr(wp), _ptr(bp), _ptr(ln_w), _ptr(ln_b), _ptr(w1), _ptr(b1),
-                                  _ptr(w2), _ptr(b2), _ptr(out), M, C, _stream()), "occ_swin_proj_ffn")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_swin_proj_ffn", att, tok, wp, bp, ln_w, ln_b, w1, b1, w2, b2, out, M, C)
     return out
 
 
@@ -450,18 +437,15 @@ def gn_apply(x, stats, w, b, rows_per_batch, groups, residual=None, relu=True, w
     if split_into is None and want_split:
         split_into = torch.empty_like(x)
     ldo = split_into.shape[1] if split_into is not None else C
-    check(lib().occ_gn_apply(_ptr(x), _ptr(stats), _ptr(w), _ptr(b), _ptr(residual), _ptr(out), _ptr(split_into), rows,
-                             rows_per_batch, C, groups, ldo, out_off, int(relu), _stream(x)), "occ_gn_apply")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_gn_apply", x, stats, w, b, residual, out, split_into, rows, rows_per_batch, C, groups, ldo, out_off,
+          int(relu))
     return out, split_into
 
 
 def aspp_gap_branch(x, wconv, gw, gb, cat, B, rows_per_batch, groups, out_off):
     ch = x.shape[1]
     sums = torch.empty((B, ch * 3 // 2 + 2), dtype=torch.float64, device=x.device)  # B*ch doubles + B*ch floats
-    check(lib().occ_aspp_gap_branch(_ptr(x), _ptr(sums), _ptr(wconv), _ptr(gw), _ptr(gb), _ptr(cat), B, rows_per_batch,
-                                    ch, groups, cat.shape[1], out_off, _stream()), "occ_aspp_gap_branch")
-    LAUNCH_COUNT[0] += 4
+    _call("occ_aspp_gap_branch", x, sums, wconv, gw, gb, cat, B, rows_per_batch, ch, groups, cat.shape[1], out_off)
     return cat
 
 
@@ -470,10 +454,8 @@ def dualpath_fuse(x, bev, cw, cbias, identity, B, XY, Z, C, identity_split=False
     """-> (out fp32 | None, out S32 | None), each (B*XY*Z, C)."""
     out = torch.empty((B * XY * Z, C), dtype=torch.float32, device=x.device) if want_f32 else None
     out_s = torch.empty((B * XY * Z, C), dtype=torch.float32, device=x.device) if want_split else None
-    check(lib().occ_dualpath_fuse(_ptr(x), _ptr(bev), _ptr(cw), float(cbias), _ptr(identity), int(identity_split),
-                                  _ptr(id_stats), _ptr(id_w), _ptr(id_b), groups, _ptr(out), _ptr(out_s), B, XY, Z, C,
-                                  _stream(x)), "occ_dualpath_fuse")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_dualpath_fuse", x, bev, cw, float(cbias), identity, int(identity_split), id_stats, id_w, id_b, groups,
+          out, out_s, B, XY, Z, C)
     return out, out_s
 
 
@@ -489,9 +471,7 @@ def window_attention(qkv, qkv_bias, bias_pad, B, X, Y, Z, C, heads, shift, head_
     rows = B * X * Y * (Z + 1)
     assert qkv.shape == (rows, 3 * C)
     out = torch.empty((rows, C), dtype=torch.float32, device=qkv.device)
-    check(lib().occ_window_attention(_ptr(qkv), _ptr(qkv_bias), _ptr(bias_pad), _ptr(out), B, X, Y, Z, C, heads,
-                                     int(shift), int(head_major), _stream()), "occ_window_attention")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_window_attention", qkv, qkv_bias, bias_pad, out, B, X, Y, Z, C, heads, int(shift), int(head_major))
     return out
 
 
@@ -503,17 +483,14 @@ def swin_qkv_attention(tokn_wl, w_qkv, b_qkv, bias_pad, B, X, Y, Z, C, heads, sh
     rows = B * X * Y * (Z + 1)
     assert tokn_wl.shape == (lib().occ_window_layout_rows(B, X, Y, Z), C) and w_qkv.shape == (3 * C, C)
     out = torch.empty((rows, C), dtype=torch.float32, device=tokn_wl.device)
-    check(lib().occ_swin_qkv_attention(_ptr(tokn_wl), _ptr(w_qkv), _ptr(b_qkv), _ptr(bias_pad), _ptr(out), B, X, Y, Z, C, heads,
-                                       int(shift), _stream(tokn_wl)), "occ_swin_qkv_attention")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_swin_qkv_attention", tokn_wl, w_qkv, b_qkv, bias_pad, out, B, X, Y, Z, C, heads, int(shift))
     return out
 
 
 # ----------------------------------------------------------------------------------------------- decoder head
 def sine_pos3d(X, Y, Z, num_feats, device, temperature=10000.0, scale=6.283185307179586, eps=1e-6, offset=0.0):
     out = torch.empty((X * Y * Z, 3 * num_feats), dtype=torch.float32, device=device)
-    check(lib().occ_sine_pos3d(_ptr(out), X, Y, Z, num_feats, temperature, scale, eps, offset, _stream()), "occ_sine_pos3d")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_sine_pos3d", out, X, Y, Z, num_feats, temperature, scale, eps, offset)
     return out
 
 
@@ -526,9 +503,7 @@ def head_prep(x, channel_last, level_embed=None, pos=None):
         B, C, S = x.shape
     mem = torch.empty((B, S, C), dtype=torch.float32, device=x.device)
     kpos = torch.empty_like(mem) if pos is not None else None
-    check(lib().occ_head_prep(_ptr(x), int(channel_last), _ptr(level_embed), _ptr(pos), _ptr(mem), _ptr(kpos), B, S, C,
-                              _stream()), "occ_head_prep")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_head_prep", x, int(channel_last), level_embed, pos, mem, kpos, B, S, C)
     return mem, kpos
 
 
@@ -542,13 +517,9 @@ def query_head(query_in, W, NC, norm2=None, next_q=None, ffn_part=None):
     qh = torch.empty_like(query_in) if next_q is not None else None
     n2w, n2b = norm2 if norm2 is not None else (None, None)
     qpos, Q, wqT, bq, scale = next_q if next_q is not None else (None, 0, None, None, 0.0)
-    check(lib().occ_query_head(_ptr(query_in), _ptr(n2w), _ptr(n2b), _ptr(query) if norm2 is not None else None,
-                               _ptr(W["pn_w"]), _ptr(W["pn_b"]), _ptr(W["clsT"]), _ptr(W["cls_b"]), NC, _ptr(W["m0T"]),
-                               _ptr(W["m0b"]), _ptr(W["m1T"]), _ptr(W["m1b"]), _ptr(W["m2T"]), _ptr(W["m2b"]), _ptr(cls),
-                               _ptr(membed), _ptr(qpos), Q, _ptr(wqT), _ptr(bq), scale, _ptr(qh), _ptr(ffn_part),
-                               ffn_part.shape[0] if ffn_part is not None else 0, rows, E, _stream()),
-          "occ_query_head")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_query_head", query_in, n2w, n2b, query if norm2 is not None else None, W["pn_w"], W["pn_b"], W["clsT"],
+          W["cls_b"], NC, W["m0T"], W["m0b"], W["m1T"], W["m1b"], W["m2T"], W["m2b"], cls, membed, qpos, Q, wqT, bq,
+          scale, qh, ffn_part, ffn_part.shape[0] if ffn_part is not None else 0, rows, E)
     return cls, membed, query, qh
 
 
@@ -564,8 +535,7 @@ def mask_pool(mask, B, grid, out_grid, Q):
     Xo, Yo, Zo = out_grid
     pooled = torch.empty((B, Xo * Yo * Zo, Q), dtype=torch.int32, device=mask.device)
     flag = torch.empty((B * Q,), dtype=torch.int32, device=mask.device)
-    check(lib().occ_mask_pool(_ptr(mask), _ptr(pooled), _ptr(flag), B, X, Y, Z, Xo, Yo, Zo, Q, _stream()), "occ_mask_pool")
-    LAUNCH_COUNT[0] += 2
+    _call("occ_mask_pool", mask, pooled, flag, B, X, Y, Z, Xo, Yo, Zo, Q)
     return pooled, flag
 
 
@@ -578,12 +548,11 @@ def mask_gemm_pool(mf_r, membed, B, grid, out_grid, Q):
     E = mf_r.shape[-1]
     pooled = torch.empty((B, Xo * Yo * Zo, Q), dtype=torch.int32, device=mf_r.device)
     flag = torch.empty((B * Q,), dtype=torch.int32, device=mf_r.device)
-    rc = lib().occ_mask_gemm_pool(_ptr(mf_r), _ptr(membed), _ptr(pooled), _ptr(flag), B, X, Y, Z, E, Q, Xo, Yo, Zo,
-                                  _stream())
+    rc = lib().occ_mask_gemm_pool(mf_r.data_ptr(), membed.data_ptr(), pooled.data_ptr(), flag.data_ptr(), B, X, Y, Z, E,
+                                  Q, Xo, Yo, Zo, _stream())
     if rc == -2:  # OCC_EUNSUPPORTED
         return None
     check(rc, "occ_mask_gemm_pool")
-    LAUNCH_COUNT[0] += 3 if X // Xo == 8 else 2  # flag memset [+ pooled memset for 8-voxel windows] + kernel
     return pooled, flag
 
 
@@ -592,10 +561,8 @@ def cross_attn_tc(qh, Kp, Vp, ld, koff, voff, pooled, flag, B, S, Q, E, H):
     npart = lib().occ_cross_attn_tc_partials(S)
     part = torch.empty((B, H, npart, Q, 34), dtype=torch.float32, device=qh.device)
     bits = torch.empty((B, 4 * ((S + 127) // 128), Q), dtype=torch.int32, device=qh.device)
-    check(lib().occ_mask_bits(_ptr(pooled), _ptr(bits), B, S, Q, _stream()), "occ_mask_bits")
-    check(lib().occ_cross_attn_tc(_ptr(qh), _ptr(Kp), _ptr(Vp), ld, koff, voff, _ptr(bits), _ptr(flag), _ptr(part), B, S, Q,
-                                  E, H, _stream()), "occ_cross_attn_tc")
-    LAUNCH_COUNT[0] += 2
+    _call("occ_mask_bits", pooled, bits, B, S, Q)
+    _call("occ_cross_attn_tc", qh, Kp, Vp, ld, koff, voff, bits, flag, part, B, S, Q, E, H)
     return part, npart
 
 
@@ -603,10 +570,8 @@ def cross_merge(part, nchunk, H, query, query_pos, Q, L, scale):
     rows, E = query.shape
     q1 = torch.empty_like(query)
     sa = torch.empty((rows, 3 * E), dtype=torch.float32, device=query.device)
-    check(lib().occ_cross_merge(_ptr(part), nchunk, H, _ptr(query), _ptr(query_pos), Q, _ptr(L["ca_woT"]), _ptr(L["ca_bo"]),
-                                _ptr(L["n0w"]), _ptr(L["n0b"]), _ptr(L["sa_inT"]), _ptr(L["sa_inb"]), scale, _ptr(q1),
-                                _ptr(sa), rows, E, _stream()), "occ_cross_merge")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_cross_merge", part, nchunk, H, query, query_pos, Q, L["ca_woT"], L["ca_bo"], L["n0w"], L["n0b"],
+          L["sa_inT"], L["sa_inb"], scale, q1, sa, rows, E)
     return q1, sa
 
 
@@ -619,10 +584,8 @@ def self_attn_ffn(sa, q1, Q, L, H, nkeys=None):
     ybuf = torch.empty_like(q1)
     F = L["f1b"].numel()
     part = torch.empty((F // E, rows, E), dtype=torch.float32, device=q1.device)
-    check(lib().occ_self_attn_ffn(_ptr(sa), _ptr(q1), Q, Q if nkeys is None else nkeys, _ptr(L["sa_woT"]), _ptr(L["sa_bo"]), _ptr(L["n1w"]), _ptr(L["n1b"]),
-                                  _ptr(L["f1T"]), _ptr(L["f1b"]), _ptr(L["f2T"]), _ptr(L["f2b"]), F, _ptr(x1), _ptr(ybuf),
-                                  _ptr(part), rows, E, H, _stream()), "occ_self_attn_ffn")
-    LAUNCH_COUNT[0] += 2
+    _call("occ_self_attn_ffn", sa, q1, Q, Q if nkeys is None else nkeys, L["sa_woT"], L["sa_bo"], L["n1w"], L["n1b"],
+          L["f1T"], L["f1b"], L["f2T"], L["f2b"], F, x1, ybuf, part, rows, E, H)
     return ybuf, part
 
 
@@ -633,9 +596,7 @@ def classmix(mask, cls, B, grid, out_grid, Q, NC, with_labels=False):
     Xo, Yo, Zo = out_grid
     out = torch.empty((B, NC - 1, Xo, Yo, Zo), dtype=torch.float32, device=mask.device)
     labels = torch.empty((B, Xo, Yo, Zo), dtype=torch.uint8, device=mask.device) if with_labels else None
-    check(lib().occ_classmix(_ptr(mask), mask.shape[-1], _ptr(cls), _ptr(out), _ptr(labels), B, X, Y, Z, Xo, Yo, Zo, Q, NC, _stream()),
-          "occ_classmix")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_classmix", mask, mask.shape[-1], cls, out, labels, B, X, Y, Z, Xo, Yo, Zo, Q, NC)
     return (out, labels) if with_labels else out
 
 
@@ -665,9 +626,8 @@ def panoptic_voxels(mask, cls, B, grid, out_grid, Q, thing, point_rule=False):
     sem = torch.empty((B, Xo, Yo, Zo), dtype=torch.int64, device=mask.device)
     pan = torch.empty_like(sem)
     qidx, present, table = _panoptic_ws(B, Xo * Yo * Zo, Qs, mask.device)
-    check(lib().occ_panoptic_voxels(_ptr(mask), Qs, _ptr(cls), B, X, Y, Z, Xo, Yo, Zo, Q, NC, thing, int(point_rule), _ptr(qidx),
-                                    _ptr(present), _ptr(table), _ptr(sem), _ptr(pan), _stream(mask)), "occ_panoptic_voxels")
-    LAUNCH_COUNT[0] += 4
+    _call("occ_panoptic_voxels", mask, Qs, cls, B, X, Y, Z, Xo, Yo, Zo, Q, NC, thing, int(point_rule), qidx, present,
+          table, sem, pan)
     return sem, pan
 
 
@@ -685,17 +645,14 @@ def panoptic_points(mask, cls, B, grid, Q, thing, pts, pc_range, border=True):
     pan = torch.zeros_like(sem)
     qidx, present, table = _panoptic_ws(B, n, Qs, mask.device)
     r = [float(v) for v in pc_range]
-    check(lib().occ_panoptic_points(_ptr(mask), Qs, _ptr(cls), B, X, Y, Z, Q, NC, thing, _ptr(pts), pts.shape[2], n, *r,
-                                    int(border), _ptr(qidx), _ptr(present), _ptr(table), _ptr(sem), _ptr(pan),
-                                    _stream(mask)), "occ_panoptic_points")
-    LAUNCH_COUNT[0] += 4 if n else 0
+    _call("occ_panoptic_points", mask, Qs, cls, B, X, Y, Z, Q, NC, thing, pts, pts.shape[2], n, *r, int(border), qidx,
+          present, table, sem, pan)
     return sem, pan
 
 
 def transpose_sq(mask, B, S, Q):
     out = torch.empty((B, Q, S), dtype=torch.float32, device=mask.device)
-    check(lib().occ_transpose_sq(_ptr(mask), _ptr(out), B, S, Q, _stream()), "occ_transpose_sq")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_transpose_sq", mask, out, B, S, Q)
     return out
 
 
@@ -707,9 +664,8 @@ def lidarseg_points(vox, pts, pc_range, border=True):
     n = pts.shape[0]
     out = torch.empty((n, K), dtype=torch.float32, device=vox.device)
     r = [float(v) for v in pc_range]
-    check(lib().occ_lidarseg_points(_ptr(vox), _ptr(pts) if n else None, pts.shape[1] if n else 3, n, r[0], r[1], r[2],
-                                    r[3], r[4], r[5], X, Y, Z, K, int(border), _ptr(out), _stream()), "occ_lidarseg_points")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_lidarseg_points", vox, pts if n else None, pts.shape[1] if n else 3, n, r[0], r[1], r[2], r[3], r[4],
+          r[5], X, Y, Z, K, int(border), out)
     return out
 
 
@@ -724,8 +680,7 @@ def gn_stats(x, B, rows_per_batch, C, groups):
     -> (B, groups, 2); for a conv whose bias comes before the GroupNorm (the epilogue statistics are of the raw output)."""
     _chk(x, "x")
     stats = torch.zeros((B, groups, 2), dtype=torch.float64, device=x.device)
-    check(lib().occ_gn_stats(_ptr(x), _ptr(stats), B, rows_per_batch, C, C // groups, _stream(x)), "occ_gn_stats")
-    LAUNCH_COUNT[0] += 2
+    _call("occ_gn_stats", x, stats, B, rows_per_batch, C, C // groups)
     return stats
 
 
@@ -737,9 +692,7 @@ def neck_token_prep(x, grids, B, ln=None, pos=None, want_f32=True, want_s32=True
     s32 = torch.empty_like(x) if want_s32 else None
     ps = torch.empty_like(x) if want_pos else None
     lw, lb = ln if ln is not None else (None, None)
-    check(lib().occ_neck_token_prep(_ptr(x), _ptr(lw), _ptr(lb), _ptr(pos), _ptr(f32), _ptr(s32), _ptr(ps), len(grids), B,
-                                    _grids_arr(grids), C, _stream(x)), "occ_neck_token_prep")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_neck_token_prep", x, lw, lb, pos, f32, s32, ps, len(grids), B, _grids_arr(grids), C)
     return f32, s32, ps
 
 
@@ -750,9 +703,8 @@ def ms_deform_attn(value, ow, grids, strides, B, E, H, P):
     assert value.shape[1] % H == 0 and value.shape[1] // H >= E // H
     out = torch.empty(value.shape[0], E, dtype=torch.float32, device=value.device)
     st = (ctypes.c_float * len(strides))(*[float(v) for v in strides])
-    check(lib().occ_ms_deform_attn(_ptr(value), value.shape[1], value.shape[1] // H, _ptr(ow), _ptr(out), len(grids), B,
-                                   _grids_arr(grids), st, E, H, P, _stream(value)), "occ_ms_deform_attn")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_ms_deform_attn", value, value.shape[1], value.shape[1] // H, ow, out, len(grids), B, _grids_arr(grids),
+          st, E, H, P)
     return out
 
 
@@ -777,9 +729,7 @@ def gn_upsample_add(cur, stats, gw, gb, groups, coarse):
     B, X, Y, Z, C = cur.shape
     _, Xc, Yc, Zc, _ = coarse.shape
     out = torch.empty_like(cur)
-    check(lib().occ_gn_upsample_add(_ptr(cur), _ptr(stats), _ptr(gw), _ptr(gb), groups, _ptr(coarse), _ptr(out), B, X, Y, Z,
-                                    Xc, Yc, Zc, C, _stream(cur)), "occ_gn_upsample_add")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_gn_upsample_add", cur, stats, gw, gb, groups, coarse, out, B, X, Y, Z, Xc, Yc, Zc, C)
     return out
 
 
@@ -791,8 +741,7 @@ def ssc_counts(pred, target, K, ignore=255):
     assert p.numel() == t.numel()
     ws = torch.empty(K * K, dtype=torch.int64, device=p.device)
     out = torch.empty(3 + 3 * K, dtype=torch.int64, device=p.device)
-    check(lib().occ_ssc_counts(_ptr(p), _ptr(t), p.numel(), K, ignore, _ptr(ws), _ptr(out), _stream(p)), "occ_ssc_counts")
-    LAUNCH_COUNT[0] += 2
+    _call("occ_ssc_counts", p, t, p.numel(), K, ignore, ws, out)
     return out
 
 
@@ -833,9 +782,7 @@ def panoptic_eval(x_sem, x_inst, y_sem, y_inst, K, ignore_mask, min_points, stat
     _chk(state, "state", torch.int64)
     assert state.numel() == K * K + 6 * K + 1, "panoptic state vector has the wrong length"
     ws = _panoptic_eval_ws(n, xs.device)
-    check(lib().occ_panoptic_eval(_ptr(xs), _ptr(xi), _ptr(ys), _ptr(yi), n, K, ignore_mask, min_points, parts, _ptr(ws),
-                                  ws.numel(), _ptr(state), _stream(xs)), "occ_panoptic_eval")
-    LAUNCH_COUNT[0] += 0 if n == 0 else (5 if parts & 2 else 3)  # memset, scan, [pair, segment,] fold
+    _call("occ_panoptic_eval", xs, xi, ys, yi, n, K, ignore_mask, min_points, parts, ws, ws.numel(), state)
     return state
 
 
@@ -844,7 +791,5 @@ def lidarseg_hist(scores, labels, K, hist=None):
     labels = _chk(labels.long().contiguous(), "labels", torch.int64)
     if hist is None:
         hist = torch.zeros((K - 1, K - 1), dtype=torch.int64, device=scores.device)
-    check(lib().occ_lidarseg_hist(_ptr(scores), _ptr(labels), scores.shape[0], K, _ptr(hist), _stream(scores)),
-          "occ_lidarseg_hist")
-    LAUNCH_COUNT[0] += 1
+    _call("occ_lidarseg_hist", scores, labels, scores.shape[0], K, hist)
     return hist

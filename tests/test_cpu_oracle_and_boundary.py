@@ -148,7 +148,7 @@ def test_product_does_not_import_oracle():
 
 
 # ------------------------------------------------------------------ C ABI
-def test_library_exports_every_declared_symbol():
+def test_library_binds_every_declaration_with_its_header_types():
     from occformer_b200 import _lib
     assert os.path.exists(_lib.LIB_PATH), "libocc_b200.so not built (python -m occformer_b200.build)"
     l = _lib.lib()  # sets argtypes for every symbol, AttributeError if one is missing
@@ -156,13 +156,46 @@ def test_library_exports_every_declared_symbol():
     declared = set(re.findall(r"\b(occ_[a-z0-9_]+)\s*\(", header))
     declared -= {"occ_stream_t"}
     assert declared, "no declarations parsed"
+    sigs = _lib.signatures()
+    assert set(sigs) == declared, "the ctypes binding skipped a declaration"
     for name in declared:
         assert hasattr(l, name), f"{name} declared in include/occ_b200.h but not exported"
-        assert name in _lib.SIGNATURES, f"{name} has no ctypes signature"
-    assert set(_lib.SIGNATURES) == declared
+        fn = getattr(l, name)
+        assert (fn.restype, list(fn.argtypes)) == sigs[name], f"{name}: bound types differ from its declaration"
     assert l.occ_version() >= 100
     # pure host-side helper (no GPU needed)
     assert l.occ_voxel_pool_workspace_bytes(1000, 1, 10, 10, 2) > (200 + 201 + 2000) * 4
+
+
+def test_header_parser_types(tmp_path):
+    """_lib.signatures on the declarations that need more than `int` / pointer: multi-word integer types, a comment
+    inside a parameter list, (void); an unknown type or a missing header raises."""
+    from ctypes import c_float, c_int, c_longlong, c_size_t, c_uint, c_ulonglong, c_void_p as P
+    from occformer_b200 import _lib
+    sigs = _lib.signatures()
+    assert sigs["occ_version"] == (c_int, [])
+    assert sigs["occ_launch_count"] == (c_longlong, [])
+    assert sigs["occ_window_layout_rows"] == (c_longlong, [c_int] * 4)
+    assert sigs["occ_panoptic_eval_workspace_bytes"] == (c_size_t, [c_longlong])
+    assert sigs["occ_panoptic_eval"] == (c_int, [P] * 4 + [c_longlong, c_int, c_uint, c_int, c_int, P, c_size_t, P, P])
+    assert sigs["occ_panoptic_voxels"] == (c_int, [P, c_int, P] + [c_int] * 9 + [c_ulonglong, c_int] + [P] * 5 + [P])
+    assert sigs["occ_query_head"] == (c_int, [P] * 8 + [c_int] + [P] * 9 + [c_int, P, P, c_float, P, P] + [c_int] * 3 +
+                                      [P])
+    bad = tmp_path / "bad.h"
+    bad.write_text("int occ_ok(const float* x /* (n, C) */, int n);\nshort occ_bad(int a);\n")
+    with pytest.raises(RuntimeError, match="occ_bad"):
+        _lib.signatures(str(bad))
+    with pytest.raises(RuntimeError, match="missing"):
+        _lib.signatures(str(tmp_path / "absent.h"))
+
+
+def test_rejected_call_enqueues_nothing():
+    """An argument error returns -1 before any launch: the library's launch count does not move (no GPU needed)."""
+    from occformer_b200 import _lib
+    l = _lib.lib()
+    n0 = l.occ_launch_count()
+    assert l.occ_gemm_bf16x3(None, None, None, 1, 1, 32, None, None, 0, 0, None) == -1
+    assert l.occ_launch_count() == n0
 
 
 def test_qkv_head_major_permutation_matches_reference_split():
