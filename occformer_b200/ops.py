@@ -1,13 +1,14 @@
 """Torch-tensor wrappers over the C-ABI kernels (device memory + streams are torch's; the math is ours).
 
-Every function checks device / dtype / contiguity, passes raw pointers and the current torch stream to
-libocc_b200.so and raises RuntimeError on a non-zero return code.  No fallback paths.
+Every call checks each tensor argument against its pointer declaration in include/occ_b200.h (CUDA, current device,
+dtype, contiguity), passes raw pointers and the current torch stream to libocc_b200.so and raises RuntimeError on a
+non-zero return code.  No fallback paths.
 """
 import ctypes
 
 import torch
 
-from ._lib import check, lib
+from ._lib import check, lib, parameters
 
 
 class _LaunchCount:
@@ -24,27 +25,42 @@ LAUNCH_COUNT = _LaunchCount()
 
 
 def _stream():
-    """the current torch stream of the current device (where _chk requires a call's tensors to live)"""
+    """the current torch stream of the current device (where _checked requires a call's tensors to live)"""
     return torch.cuda.current_stream().cuda_stream
 
 
-def _call(name, *args):
-    """lib().<name>(*args, current stream) with tensors passed as device pointers and None as NULL; raises RuntimeError
-    on a non-zero return code."""
-    check(getattr(lib(), name)(*(a.data_ptr() if torch.is_tensor(a) else a for a in args), _stream()), name)
+# tensor dtype per pointee type of the header (S32 is a float32 container; void: any; size_t* is host-only: no tensor)
+_DTYPES = {"float": torch.float32, "double": torch.float64, "long long": torch.int64, "int": torch.int32,
+           "unsigned": torch.int32, "unsigned int": torch.int32, "unsigned char": torch.uint8, "void": None}
 
 
-def _chk(t, name, dtype=torch.float32):
+def _checked(t, fn, i, strided=False):
+    """tensor t as parameter i of fn, checked against its declaration in the header: a pointer whose pointee type matches
+    t's dtype, t a contiguous (unless strided: the caller passes its strides) CUDA tensor on the current device -> t"""
+    param, pointee = parameters()[fn][i]
+    what = f"occformer_b200: {fn}({param})"
+    if pointee not in _DTYPES:
+        raise RuntimeError(f"{what} is not a device pointer and cannot take a tensor")
     if not t.is_cuda:
-        raise RuntimeError(f"occformer_b200: {name} must be a CUDA tensor (no CPU fallback exists)")
-    if t.dtype != dtype:
-        raise RuntimeError(f"occformer_b200: {name} must be {dtype}, got {t.dtype}")
-    if not t.is_contiguous():
-        raise RuntimeError(f"occformer_b200: {name} must be contiguous")
+        raise RuntimeError(f"{what} must be a CUDA tensor (no CPU fallback exists)")
     if t.device.index != torch.cuda.current_device():
-        raise RuntimeError(f"occformer_b200: {name} lives on {t.device} but the current device is "
-                           f"cuda:{torch.cuda.current_device()} (wrap the call in torch.cuda.device(...))")
+        raise RuntimeError(f"{what} lives on {t.device} but the current device is cuda:{torch.cuda.current_device()} "
+                           "(wrap the call in torch.cuda.device(...))")
+    if _DTYPES[pointee] not in (None, t.dtype):
+        raise RuntimeError(f"{what} must be {_DTYPES[pointee]}, got {t.dtype}")
+    if not (strided or t.is_contiguous()):
+        raise RuntimeError(f"{what} must be contiguous")
     return t
+
+
+def _call(name, *args, unsupported_ok=False):
+    """lib().<name>(*args, current stream) with tensors checked and passed as device pointers and None as NULL -> its return
+    code; raises RuntimeError if that is not 0 (or -2, unsupported shape with nothing enqueued, when unsupported_ok)"""
+    args = [_checked(a, name, i).data_ptr() if torch.is_tensor(a) else a for i, a in enumerate(args)]
+    rc = getattr(lib(), name)(*args, _stream())
+    if not (unsupported_ok and rc == -2):
+        check(rc, name)
+    return rc
 
 
 # ----------------------------------------------------------------------------------------------- S32 split format
@@ -97,7 +113,6 @@ def unsplit_weight(ws):
 
 def to_split(x):
     """fp32 CUDA tensor (..., C), C % 32 == 0 -> S32 (device kernel)."""
-    _chk(x, "x")
     C = x.shape[-1]
     out = torch.empty_like(x)
     _call("occ_split_rows", x, out, x.numel() // C, C)
@@ -105,7 +120,6 @@ def to_split(x):
 
 
 def from_split(x):
-    _chk(x, "x")
     C = x.shape[-1]
     out = torch.empty_like(x)
     _call("occ_unsplit_rows", x, out, x.numel() // C, C)
@@ -178,7 +192,7 @@ def lss_geometry(frustum, rots, trans, intrins, post_rots, post_trans, bda):
     """frustum (D,fH,fW,3) + camera matrices -> geom (B,N,D,fH,fW,3)."""
     B, N = trans.shape[:2]
     D, fH, fW, _ = frustum.shape
-    f = lambda t: _chk(t.float().contiguous(), "camera matrix")  # noqa: E731
+    f = lambda t: t.float().contiguous()  # noqa: E731
     geom = torch.empty((B, N, D, fH, fW, 3), dtype=torch.float32, device=frustum.device)
     fr, r, t, k, pr, pt, bd = f(frustum), f(rots), f(trans), f(intrins), f(post_rots), f(post_trans), f(bda)
     _call("occ_lss_geometry", fr, D * fH * fW, r, t, k, k.shape[-2], k.shape[-1], pr, pt, bd, bd.shape[-1], B, N, geom)
@@ -187,7 +201,6 @@ def lss_geometry(frustum, rots, trans, intrins, post_rots, post_trans, bda):
 
 def lift_prologue(depth_logits, img_feat):
     """depth_logits (BN,D,fH,fW), img_feat (BN,C,fH,fW) -> depth_prob (BN,D,fH,fW), feat_cl (BN,fH*fW,C)."""
-    _chk(depth_logits, "depth_logits"), _chk(img_feat, "img_feat")
     BN, D, fH, fW = depth_logits.shape
     C = img_feat.shape[1]
     prob = torch.empty_like(depth_logits)
@@ -198,7 +211,6 @@ def lift_prologue(depth_logits, img_feat):
 
 def lift_splat(depth_prob, feat_cl, geom, B, N, dx, bx, nx, grid, return_workspace=False, with_split=False):
     """Fused lift-splat.  Returns the channel-last grid (B,X,Y,Z,C) [, its S32 copy when with_split]."""
-    _chk(depth_prob, "depth_prob"), _chk(feat_cl, "feat_cl"), _chk(geom, "geom")
     BN, D, fH, fW = depth_prob.shape
     C = feat_cl.shape[-1]
     X, Y, Z = grid
@@ -222,17 +234,15 @@ def lift_splat_fused(depth_logits, img_feat, frustum, rots, trans, intrins, post
     X, Y, Z = grid
     HW = fH * fW
 
-    def plane(t, name):  # (BN, ch, fH, fW) fp32 whose cameras may be strided (channel slice of a bigger tensor): no copy
+    def plane(t, i):  # (BN, ch, fH, fW) fp32 whose cameras may be strided (channel slice of a bigger tensor): no copy
         t = t.float()
         if t.stride()[1:] != (HW, fW, 1):
             t = t.contiguous()
-        if not t.is_cuda:
-            raise RuntimeError(f"occformer_b200: {name} must be a CUDA tensor (no CPU fallback exists)")
-        return t, t.stride(0)
+        return t, _checked(t, "occ_lift_splat_fused", i, strided=True).data_ptr(), t.stride(0)
 
-    depth_logits, ls = plane(depth_logits, "depth_logits")
-    img_feat, fs = plane(img_feat, "img_feat")
-    f = lambda t: _chk(t.float().contiguous(), "camera matrix")  # noqa: E731
+    depth_logits, lp, ls = plane(depth_logits, 0)  # keeps a copy alive: the allocations below must not reuse it
+    img_feat, fp, fs = plane(img_feat, 2)
+    f = lambda t: t.float().contiguous()  # noqa: E731
     fr, r, t, k, pr, pt, bd = f(frustum), f(rots), f(trans), f(intrins), f(post_rots), f(post_trans), f(bda)
     dev = depth_logits.device
     ws = _workspace(BN * D * HW, B, X, Y, Z, dev)
@@ -241,14 +251,13 @@ def lift_splat_fused(depth_logits, img_feat, frustum, rots, trans, intrins, post
     out = torch.empty((B, X, Y, Z, C), dtype=torch.float32, device=dev)
     out_s = torch.empty_like(out) if with_split else None
     fl = [float(v) for v in (*dx, *bx, *nx)]
-    _call("occ_lift_splat_fused", depth_logits, ls, img_feat, fs, fr, r, t, k, k.shape[-2], k.shape[-1], pr, pt, bd,
+    _call("occ_lift_splat_fused", lp, ls, fp, fs, fr, r, t, k, k.shape[-2], k.shape[-1], pr, pt, bd,
           bd.shape[-1], prob, feat_cl, out, out_s, B, N, D, HW, C, *fl, X, Y, Z, ws.buf, ws.nbytes)
     return ((out, out_s) if with_split else out), prob
 
 
 def voxel_pool_geom(feats, geom, B, dx, bx, nx, grid, return_workspace=False):
     """Materialised-volume voxel pooling: feats (P,C), geom (P,3) -> (B,X,Y,Z,C)."""
-    _chk(feats, "feats"), _chk(geom, "geom")
     P_, C = feats.shape
     X, Y, Z = grid
     ws = _workspace(P_, B, X, Y, Z, feats.device)
@@ -259,7 +268,6 @@ def voxel_pool_geom(feats, geom, B, dx, bx, nx, grid, return_workspace=False):
 
 
 def bev_pool_channel_last(feats, coords, B, X, Y, Z, return_workspace=False):
-    _chk(feats, "feats"), _chk(coords, "coords", torch.int64)
     n, C = feats.shape
     ws = _workspace(n, B, X, Y, Z, feats.device)
     out = torch.empty((B, X, Y, Z, C), dtype=torch.float32, device=feats.device)
@@ -271,18 +279,12 @@ def bev_pool_channel_last(feats, coords, B, X, Y, Z, return_workspace=False):
 def gemm(a, w, bias=None, residual=None, act=0, split_out=False, out=None):
     """out[M,N] = act(a[M,K] @ w[N,K]^T + bias) (+ residual).  a, w in S32 (to_split / split_weight / a producer's
     split output); out fp32, or S32 when split_out (operand of the next contraction)."""
-    _chk(a, "a"), _chk(w, "w")
     M, K = a.shape
     N = w.shape[0]
     assert w.shape[1] == K
     if out is None:
         out = torch.empty((M, N), dtype=torch.float32, device=a.device)
-    else:
-        _chk(out, "out")
-    if bias is not None:
-        _chk(bias, "bias")
     if residual is not None:
-        _chk(residual, "residual")
         assert residual.shape == (M, N)
     _call("occ_gemm_bf16x3", a, w, out, M, N, K, bias, residual, act, int(split_out))
     return out
@@ -301,7 +303,6 @@ def conv(x_cl, w2, ksize, stride=1, dil=1, bias=None, residual=None, act=0, spli
     """x_cl (B,X,Y,Z,Cin) channel-last S32; w2 from repack_conv_weight; returns (B,Xo,Yo,Zo,Cout) channel-last raw
     output (fp32, or S32 when split_out).  gn_stats: zero-initialised double tensor (B, groups, 2) receiving (sum, sumsq)
     of the raw output, cpg = Cout // groups channels per group (any cpg, at most 96 groups)."""
-    _chk(x_cl, "x_cl"), _chk(w2, "w2")
     B, X, Y, Z, Cin = x_cl.shape
     KX, KY, KZ = ksize
     Cout = w2.shape[0]
@@ -313,8 +314,6 @@ def conv(x_cl, w2, ksize, stride=1, dil=1, bias=None, residual=None, act=0, spli
 
     Xo, Yo, Zo = osz(X, KX), osz(Y, KY), osz(Z, KZ)
     out = torch.empty((B, Xo, Yo, Zo, Cout), dtype=torch.float32, device=x_cl.device)
-    if gn_stats is not None:
-        _chk(gn_stats, "gn_stats", torch.float64)
     ws = _conv_workspace(x_cl.device)
     _call("occ_conv_bf16x3", x_cl, w2, out, B, X, Y, Z, Cin, Cout, KX, KY, KZ, stride, dil, bias, residual, act,
           int(split_out), gn_stats, cpg, ws, ws.numel())
@@ -332,15 +331,12 @@ def conv_plan(B, X, Y, Z, Cin, Cout, ksize=(3, 3, 3), stride=1, dil=1, splitk_ok
 def conv_taps(x_cl, w2, taps, gn_stats=None, cpg=0):
     """Stride-1 convolution over an explicit tap table (several dilated branches in one launch): x_cl (B,X,Y,Z,Cin) S32,
     taps = [(dx, dy, dz), ...], w2 (Cout, len(taps)*Cin) S32 tap-major -> raw (B,X,Y,Z,Cout) fp32."""
-    _chk(x_cl, "x_cl"), _chk(w2, "w2")
     B, X, Y, Z, Cin = x_cl.shape
     Cout = w2.shape[0]
     assert w2.shape[1] == len(taps) * Cin
     out = torch.empty((B, X, Y, Z, Cout), dtype=torch.float32, device=x_cl.device)
     flat = [int(v) for t in taps for v in t]
     arr = (ctypes.c_int * len(flat))(*flat)
-    if gn_stats is not None:
-        _chk(gn_stats, "gn_stats", torch.float64)
     _call("occ_conv_taps_bf16x3", x_cl, w2, out, B, X, Y, Z, Cin, Cout, len(taps), arr, gn_stats, cpg)
     return out
 
@@ -406,7 +402,6 @@ def gn_relu_zmean_ln(y, stats, gn_w, gn_b, ln_w, ln_b, B, XY, Z, C, groups, X=0,
 
 
 def layernorm(x, w, b, split_out=False):
-    _chk(x, "x")
     rows, C = x.shape
     out = torch.empty_like(x)
     _call("occ_layernorm", x, w, b, out, rows, C, int(split_out))
@@ -415,7 +410,6 @@ def layernorm(x, w, b, split_out=False):
 
 def swin_proj_ffn(att, tok, wp, bp, ln_w, ln_b, w1, b1, w2, b2):
     """Fused Swin block tail (C == 128): tok + proj(att) -> LN2 -> FFN(GELU) + residual, one kernel."""
-    _chk(att, "att"), _chk(tok, "tok")
     M, C = att.shape
     assert tok.shape == (M, C) and wp.shape == (C, C) and w1.shape == (C, C) and w2.shape == (C, C)
     out = torch.empty_like(att)
@@ -428,11 +422,9 @@ def gn_apply(x, stats, w, b, rows_per_batch, groups, residual=None, relu=True, w
     """GroupNorm apply (+ReLU, +residual) of a raw conv output x (rows, C).  Returns (out_f32 | None, out_s32 | None):
     the fp32 result when want_f32, the S32 result written into split_into[:, out_off:out_off+C] (or a fresh (rows, C)
     tensor when want_split)."""
-    _chk(x, "x")
     rows, C = x.shape
     out = out_f32 if out_f32 is not None else (torch.empty_like(x) if want_f32 else None)
     if out is not None:
-        _chk(out, "out_f32")
         assert out.shape == x.shape
     if split_into is None and want_split:
         split_into = torch.empty_like(x)
@@ -467,7 +459,6 @@ def qkv_head_major_perm(C, heads, device=None):
 
 
 def window_attention(qkv, qkv_bias, bias_pad, B, X, Y, Z, C, heads, shift, head_major=False):
-    _chk(qkv, "qkv")
     rows = B * X * Y * (Z + 1)
     assert qkv.shape == (rows, 3 * C)
     out = torch.empty((rows, C), dtype=torch.float32, device=qkv.device)
@@ -479,7 +470,6 @@ def swin_qkv_attention(tokn_wl, w_qkv, b_qkv, bias_pad, B, X, Y, Z, C, heads, sh
     """QKV projection + (shifted) window attention in one kernel (C == 128): tokn_wl (window_layout rows, C) S32 in the
     window layout of ``shift`` (gn_relu_zmean_ln(win_shift=shift) / to_window_layout), w_qkv (3C, C) S32 and b_qkv (3C,)
     fp32 with head-major rows -> attention output (B*X*Y*(Z+1), C) S32 in token order."""
-    _chk(tokn_wl, "tokn_wl"), _chk(w_qkv, "w_qkv"), _chk(b_qkv, "b_qkv")
     rows = B * X * Y * (Z + 1)
     assert tokn_wl.shape == (lib().occ_window_layout_rows(B, X, Y, Z), C) and w_qkv.shape == (3 * C, C)
     out = torch.empty((rows, C), dtype=torch.float32, device=tokn_wl.device)
@@ -496,7 +486,6 @@ def sine_pos3d(X, Y, Z, num_feats, device, temperature=10000.0, scale=6.28318530
 
 def head_prep(x, channel_last, level_embed=None, pos=None):
     """x: (B,S,C) channel-last memory or (B,C,S) reference layout -> mem (B,S,C) [, kpos (B,S,C)] in S32."""
-    _chk(x, "x")
     if channel_last:
         B, S, C = x.shape
     else:
@@ -548,11 +537,8 @@ def mask_gemm_pool(mf_r, membed, B, grid, out_grid, Q):
     E = mf_r.shape[-1]
     pooled = torch.empty((B, Xo * Yo * Zo, Q), dtype=torch.int32, device=mf_r.device)
     flag = torch.empty((B * Q,), dtype=torch.int32, device=mf_r.device)
-    rc = lib().occ_mask_gemm_pool(mf_r.data_ptr(), membed.data_ptr(), pooled.data_ptr(), flag.data_ptr(), B, X, Y, Z, E,
-                                  Q, Xo, Yo, Zo, _stream())
-    if rc == -2:  # OCC_EUNSUPPORTED
+    if _call("occ_mask_gemm_pool", mf_r, membed, pooled, flag, B, X, Y, Z, E, Q, Xo, Yo, Zo, unsupported_ok=True) == -2:
         return None
-    check(rc, "occ_mask_gemm_pool")
     return pooled, flag
 
 
@@ -618,7 +604,6 @@ def panoptic_voxels(mask, cls, B, grid, out_grid, Q, thing, point_rule=False):
     """mask (B, S, Qs) query-last logits, cls (B, Q, NC), thing = thing_mask(...) -> (semantic, panoptic) int64
     (B, *out_grid): format_panoptic_occupancy_results of the trilinearly upsampled logits; point_rule: the label rule of
     format_panoptic_lidar_results (class 0 is never a label)."""
-    _chk(mask, "mask"), _chk(cls, "cls")
     X, Y, Z = grid
     Xo, Yo, Zo = out_grid
     Qs, NC = mask.shape[-1], cls.shape[-1]
@@ -634,11 +619,10 @@ def panoptic_voxels(mask, cls, B, grid, out_grid, Q, thing, point_rule=False):
 def panoptic_points(mask, cls, B, grid, Q, thing, pts, pc_range, border=True):
     """mask (B, S, Qs) native query-last logits, cls (B, Q, NC), pts (B, n, >=3) -> (semantic, panoptic) int64 (B, n):
     forward_lidar_panopticseg, eval branch."""
-    _chk(mask, "mask"), _chk(cls, "cls")
     X, Y, Z = grid
     Qs, NC = mask.shape[-1], cls.shape[-1]
     assert cls.shape == (B, Q, NC) and mask.shape == (B, X * Y * Z, Qs)
-    pts = _chk(pts.to(mask.device).float().contiguous(), "pts")
+    pts = pts.to(mask.device).float().contiguous()
     assert pts.dim() == 3 and pts.shape[0] == B and pts.shape[2] >= 3
     n = pts.shape[1]
     sem = torch.zeros((B, n), dtype=torch.int64, device=mask.device)
@@ -658,7 +642,6 @@ def transpose_sq(mask, B, S, Q):
 
 def lidarseg_points(vox, pts, pc_range, border=True):
     """vox (K,X,Y,Z) contiguous class volume of one sample; pts (n, >=3) -> (n, K) softmaxed point scores."""
-    _chk(vox, "vox")
     K, X, Y, Z = vox.shape
     pts = pts.float().contiguous()
     n = pts.shape[0]
@@ -678,7 +661,6 @@ def _grids_arr(grids):
 def gn_stats(x, B, rows_per_batch, C, groups):
     """fp64 (sum, sumsq) per (sample, group) of a finished tensor x (B*rows_per_batch, C), C % 4 == 0, at most 96 groups
     -> (B, groups, 2); for a conv whose bias comes before the GroupNorm (the epilogue statistics are of the raw output)."""
-    _chk(x, "x")
     stats = torch.zeros((B, groups, 2), dtype=torch.float64, device=x.device)
     _call("occ_gn_stats", x, stats, B, rows_per_batch, C, C // groups)
     return stats
@@ -686,7 +668,6 @@ def gn_stats(x, B, rows_per_batch, C, groups):
 
 def neck_token_prep(x, grids, B, ln=None, pos=None, want_f32=True, want_s32=True, want_pos=False):
     """[LayerNorm] of level-major token rows x (B*Nq, C) -> (x fp32 | None, x S32 | None, (x + pos) S32 | None)."""
-    _chk(x, "x")
     rows, C = x.shape
     f32 = torch.empty_like(x) if want_f32 else None
     s32 = torch.empty_like(x) if want_s32 else None
@@ -699,7 +680,6 @@ def neck_token_prep(x, grids, B, ln=None, pos=None, want_f32=True, want_s32=True
 def ms_deform_attn(value, ow, grids, strides, B, E, H, P):
     """3-D multi-scale deformable attention core on level-major rows -> (rows, E) in S32.  value (rows, H * head_ld): head h
     in columns [h*head_ld, h*head_ld + E/H) -- head_ld = E/H, or E/H rounded up to 32 (``pad_head_rows``)."""
-    _chk(value, "value"), _chk(ow, "ow")
     assert value.shape[1] % H == 0 and value.shape[1] // H >= E // H
     out = torch.empty(value.shape[0], E, dtype=torch.float32, device=value.device)
     st = (ctypes.c_float * len(strides))(*[float(v) for v in strides])
@@ -725,7 +705,6 @@ def pad_head_rows(w, b, H):
 
 def gn_upsample_add(cur, stats, gw, gb, groups, coarse):
     """cur (B,X,Y,Z,C) raw conv output (+ stats), coarse (B,Xc,Yc,Zc,C) fp32 -> GN(cur) + trilinear_up(coarse) in S32."""
-    _chk(cur, "cur"), _chk(coarse, "coarse")
     B, X, Y, Z, C = cur.shape
     _, Xc, Yc, Zc, _ = coarse.shape
     out = torch.empty_like(cur)
@@ -736,8 +715,8 @@ def gn_upsample_add(cur, stats, gw, gb, groups, coarse):
 # ----------------------------------------------------------------------------------------------- evaluation tail
 def ssc_counts(pred, target, K, ignore=255):
     """uint8 label volumes (any shape) -> int64 (3 + 3K,): completion tp/fp/fn, semantic tp/fp/fn per class."""
-    p = _chk(pred.reshape(-1).to(torch.uint8).contiguous(), "pred", torch.uint8)
-    t = _chk(target.reshape(-1).to(torch.uint8).contiguous(), "target", torch.uint8)
+    p = pred.reshape(-1).to(torch.uint8).contiguous()
+    t = target.reshape(-1).to(torch.uint8).contiguous()
     assert p.numel() == t.numel()
     ws = torch.empty(K * K, dtype=torch.int64, device=p.device)
     out = torch.empty(3 + 3 * K, dtype=torch.int64, device=p.device)
@@ -761,12 +740,10 @@ def _panoptic_eval_ws(n, device):
 
 
 def _flat_ids(t, name):
-    """integer (or whole-number floating) CUDA tensor of any shape -> flat contiguous int64"""
-    if not torch.is_tensor(t) or not t.is_cuda:
-        raise RuntimeError(f"occformer_b200: {name} must be a CUDA tensor (no CPU fallback exists)")
+    """integer (or whole-number floating) tensor of any shape -> flat contiguous int64"""
     if t.dtype == torch.bool or t.is_complex():
         raise RuntimeError(f"occformer_b200: {name} must hold integer ids, got {t.dtype}")
-    return _chk(t.reshape(-1).to(torch.int64).contiguous(), name, torch.int64)
+    return t.reshape(-1).to(torch.int64).contiguous()
 
 
 def panoptic_eval(x_sem, x_inst, y_sem, y_inst, K, ignore_mask, min_points, state, parts=3):
@@ -779,7 +756,6 @@ def panoptic_eval(x_sem, x_inst, y_sem, y_inst, K, ignore_mask, min_points, stat
     n = xs.numel()
     if any(t is not None and t.numel() != n for t in (ys, xi, yi)):
         raise RuntimeError("occformer_b200: panoptic_eval inputs must have the same number of elements")
-    _chk(state, "state", torch.int64)
     assert state.numel() == K * K + 6 * K + 1, "panoptic state vector has the wrong length"
     ws = _panoptic_eval_ws(n, xs.device)
     _call("occ_panoptic_eval", xs, xi, ys, yi, n, K, ignore_mask, min_points, parts, ws, ws.numel(), state)
@@ -787,8 +763,7 @@ def panoptic_eval(x_sem, x_inst, y_sem, y_inst, K, ignore_mask, min_points, stat
 
 
 def lidarseg_hist(scores, labels, K, hist=None):
-    _chk(scores, "scores")
-    labels = _chk(labels.long().contiguous(), "labels", torch.int64)
+    labels = labels.long().contiguous()
     if hist is None:
         hist = torch.zeros((K - 1, K - 1), dtype=torch.int64, device=scores.device)
     _call("occ_lidarseg_hist", scores, labels, scores.shape[0], K, hist)
