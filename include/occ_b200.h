@@ -244,19 +244,21 @@ int occ_query_head(const float* query_in, const float* n2w, const float* n2b, fl
                    float* qh_out, const float* ffn_part /*(nparts, rows, E) FFN column-block partials, added to query_in
                    in the order 0..nparts-1; may be NULL with nparts = 0*/, int nparts, int rows, int E, occ_stream_t stream);
 /* adaptive_max_pool3d of the mask logits (:463), general windows -> pooled (B, Xo*Yo*Zo, Q) as order-preserving ints
- * (see occ_mask_gemm_pool); row_flag[b*Q+q] = 1 iff some key of the row is un-blocked (pooled >= 0), else the row
- * attends everywhere (:652-653).  attn_mask == pooled < 0. */
+ * (see occ_mask_gemm_pool; a -0.0 maximum encodes as +0.0); row_flag[b*Q+q] = 1 iff some key of the row is un-blocked
+ * (code >= 0), else the row attends everywhere (:652-653).  attn_mask == code < 0. */
 int occ_mask_pool(const float* mask, int* pooled, int* row_flag, int B, int X, int Y, int Z, int Xo, int Yo, int Zo,
                   int Q, occ_stream_t stream);
 /* mask einsum fused with the attention-mask pooling (:457-466) of the intermediate decoder layers, the (B,V,Q) logits
  * never written: pooled[b,cell,q] = max over the cell of <mf[b,v,:], membed[b,q,:]> as an order-preserving int
- * (i >= 0 ? i : i ^ 0x7FFFFFFF of the float bits; blocked <=> value < 0), flag[b,q] as occ_mask_pool.  Covers cubic
+ * (i >= 0 ? i : i ^ 0x7FFFFFFF of the float bits i, except that -0.0 encodes as +0.0, i.e. 0: sigmoid(-0.0) = 0.5 is not
+ * blocked; blocked <=> code < 0), flag[b,q] as occ_mask_pool.  Covers cubic
  * windows of 2, 4 or 8 voxels (box-divisible grids, E % 32 == 0, Q <= 256); returns -2 with nothing enqueued for any other
  * shape (the caller then uses occ_gemm_bf16x3 per sample + occ_mask_pool). */
 int occ_mask_gemm_pool(const float* mf /*S32*/, const float* membed /*S32*/, int* pooled, int* flag, int B, int X, int Y,
                        int Z, int E, int Q, int Xo, int Yo, int Zo, occ_stream_t stream);
 /* masked cross attention (mmcv MultiheadAttention -> nn.MultiheadAttention, bool attn_mask) on the wgmma tensor cores
- * (128-key tiles, TMA operand loads, P in registers); qh fp32, Kp / Vp S32 (one chunk per (key, head)); writes
+ * (128-key tiles, TMA operand loads, P in registers); qh fp32, Kp / Vp S32 (one chunk per (key, head)) with row pitch
+ * ld and this layer's columns at koff / voff, all three multiples of 32 (a head's slice is one aligned chunk); writes
  * occ_cross_attn_tc_partials(S) partials per (sample, head): part (B, H, npart, Q, 34) = running max, running sum, 32
  * value accumulators */
 int occ_cross_attn_tc_partials(int S);

@@ -233,14 +233,16 @@ extern "C" int occ_cross_attn_tc_partials(int S) {
 }
 
 // qh (B,Q,E) scaled projected queries (fp32); Kp / Vp (B*S, ld) projected keys / values in S32, this layer's slice at
-// column koff / voff; bits (B, NW = 4*ceil(S/128), Q) blocked-key words from occ_mask_bits; row_flag (B*Q);
-// part (B, H, npart, Q, 34).
+// column koff / voff (ld, koff, voff multiples of 32); bits (B, NW = 4*ceil(S/128), Q) blocked-key words from
+// occ_mask_bits; row_flag (B*Q); part (B, H, npart, Q, 34).
 extern "C" int occ_cross_attn_tc(const float* qh, const float* Kp, const float* Vp, int ld, int koff, int voff,
                                  const unsigned* bits, const int* row_flag, float* part, int B, int S, int Q, int E,
                                  int H, cudaStream_t stream) {
   OCC_REQUIRE(qh && Kp && Vp && bits && row_flag && part);
   OCC_REQUIRE(B > 0 && S > 0 && Q > 0 && Q <= 256 && Q % 4 == 0 && H > 0 && E == H * XT_HD && B <= 65535 && H <= 65535);
-  OCC_REQUIRE(ld % 4 == 0 && koff % 4 == 0 && voff % 4 == 0 && koff + E <= ld && voff + E <= ld);
+  // one TMA box per (key, head) = one 32-column S32 chunk [hi | lo]: the slices must start on a chunk boundary
+  OCC_REQUIRE(ld % 32 == 0 && koff % 32 == 0 && voff % 32 == 0 && koff >= 0 && voff >= 0 && koff + E <= ld &&
+              voff + E <= ld);
   OCC_REQUIRE((reinterpret_cast<uintptr_t>(qh) & 15) == 0 && (reinterpret_cast<uintptr_t>(Kp) & 15) == 0 &&
               (reinterpret_cast<uintptr_t>(Vp) & 15) == 0);
   const int tiles = (S + XT_KEYS - 1) / XT_KEYS;

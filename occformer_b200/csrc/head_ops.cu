@@ -260,10 +260,10 @@ mask_pool_kernel(const float* __restrict__ mask, int* __restrict__ pooled, int* 
 #pragma unroll 4
         for (int z = 0; z < z1 - z0; ++z) m = fmaxf(m, __ldg(p + (size_t)z * Q));
       }
-    const int mi = __float_as_int(m);
-    pooled[(size_t)cell * Q + q] = mi >= 0 ? mi : mi ^ 0x7FFFFFFF;  // order-preserving int (sign kept)
-    // attn_mask = sigmoid(m) < 0.5  <=>  m < 0 ; a row that is blocked everywhere is un-blocked (:652-653)
-    if (!(m < 0.f)) row_flag[b * Q + q] = 1;
+    const int code = ordered_logit(m);
+    pooled[(size_t)cell * Q + q] = code;
+    // attn_mask = sigmoid(m) < 0.5  <=>  code < 0 ; a row that is blocked everywhere is un-blocked (:652-653)
+    if (code >= 0) row_flag[b * Q + q] = 1;
   }
 }
 

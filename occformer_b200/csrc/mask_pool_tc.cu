@@ -37,11 +37,6 @@ struct MaskPoolParams {
   int passes;  // tensor-core passes per 32-k block (occ_common.cuh: mma_passes)
 };
 
-__device__ __forceinline__ int ordered_int(float f) {
-  const int i = __float_as_int(f);
-  return i >= 0 ? i : i ^ 0x7FFFFFFF;
-}
-
 // P: cubic pooling window; (BX, BY, BZ): voxel box of a tile (BX*BY*BZ == 128, z fastest = B-operand row order)
 template <int P, int BX, int BY, int BZ>
 __global__ void __launch_bounds__(MP_THREADS, 1)
@@ -171,7 +166,7 @@ mask_pool_tc_kernel(const __grid_constant__ CUtensorMap tmB, const MaskPoolParam
         for (int c = 0; c < NC; ++c) {
           const int cx = c / (NCY * NCZ), cy = (c / NCZ) % NCY, cz = c % NCZ;
           int* dst = pooled_b + ((size_t)((gx0 + cx) * p.Yo + gy0 + cy) * p.Zo + gz0 + cz) * p.Q + q;
-          const int o = ordered_int(m[c]);
+          const int o = ordered_logit(m[c]);
           anypos |= o >= 0;
           if (COMPLETE) *dst = o;
           else atomicMax(dst, o);

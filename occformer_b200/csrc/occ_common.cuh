@@ -1,4 +1,4 @@
-// Shared host-side helpers of libocc_b200.so: error codes, driver entry point for TMA descriptors.
+// Shared helpers of libocc_b200.so: error codes, driver entry point for TMA descriptors, the pooled-logit encoding.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -99,6 +99,14 @@ inline int sm_count() {
       if (known__) cfg__[dev__] = (size_t)(bytes);                                                                \
     }                                                                                                             \
   } while (0)
+
+// Pooled attention-mask logit -> order-preserving int (occ_mask_pool / occ_mask_gemm_pool): the float bits for x >= +0,
+// bits ^ 0x7FFFFFFF for x < 0, so that int order is float order and "blocked" (sigmoid(x) < 0.5, i.e. x < 0) is code < 0.
+// -0.0 encodes as +0.0 (code 0): sigmoid(-0.0) = 0.5 is not blocked.  ops.decode_ordered inverts it.
+__device__ __forceinline__ int ordered_logit(float x) {
+  const int i = __float_as_int(x);
+  return i >= 0 ? i : (i == (int)0x80000000 ? 0 : i ^ 0x7FFFFFFF);
+}
 
 // Tensor-core passes per 32-k operand block: 3 = fp32-faithful (hi*hi + lo*hi + hi*lo, the default and the only mode the
 // parity gate covers), 1 = single-pass bf16 (hi*hi only; occ_set_mma_passes, csrc/config.cu).  Host-side setting, read by

@@ -144,6 +144,8 @@ def test_mask_logit_pooling_routes(cuda, grid, target, B):
     ref_pool = F.adaptive_max_pool3d(own, target).flatten(2).permute(0, 2, 1)  # (B,So,Q)
     assert torch.equal(ops.decode_ordered(pooled_i).cpu(), ref_pool), f"pooled maxima differ {grid}->{target}"
     assert torch.equal(flag.cpu().view(B, Q) != 0, (ref_pool >= 0).any(1))
+    # the all-zero query decodes to +0.0 (a -0.0 maximum is encoded as +0.0; torch.equal cannot tell the two apart)
+    assert not bool(torch.signbit(ops.decode_ordered(pooled_i).cpu()[0, :, 3]).any())
     # without the mask output (intermediate decoder layers): the query-stationary kernel of mask_pool_tc.cu (same
     # products, but a different accumulator orientation, so the comparison is against the fp64 window maxima)
     fused = ops.mask_gemm_pool(mf_s, me_s, B, grid, target, Q)
@@ -156,6 +158,7 @@ def test_mask_logit_pooling_routes(cuda, grid, target, B):
     assert_close(got, ref_pool64, 5e-5, f"query-stationary pooled maxima {grid}->{target}")
     assert torch.equal(flag2.cpu().view(B, Q) != 0, (got >= 0).any(1))
     assert torch.equal(got[0, :, 3], torch.zeros_like(got[0, :, 3]))  # the all-zero query (sample 0) pools to exactly +0
+    assert not bool(torch.signbit(got[0, :, 3]).any())
 
 
 @pytest.mark.parametrize("target", [(100, 100, 8), (50, 50, 4), (25, 25, 2)])
