@@ -175,6 +175,32 @@ int occ_deform_im2col(const float* x, const float* off, int off_ld, float* cols,
                       occ_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * Image encoder of the nuScenes R50 model (projects/configs/occformer_nusc/occformer_nusc_r50_256x704.py:65-79):
+ * img_backbone = mmdet 2.14.0 ResNet(depth=50) (mmdet/models/backbones/resnet.py), img_neck = SECONDFPN
+ * (M/models/necks/second_fpn.py:11-91), inference with eval-mode BatchNorms folded into the convolutions.  Every
+ * convolution is an occ_gemm_bf16x3 / occ_conv_bf16x3 / occ_conv_slice_bf16x3 launch; the entry points below are the
+ * layout steps those cannot do.  Activations are channel-last rows (image, y, x) of C floats. */
+/* ResNet stem conv1 (7x7, stride 2, padding 3, Cin = 3; ResNet._make_stem_layer) as im2col: img (n, 3, H, W) NCHW fp32
+ * -> cols (n*Ho*Wo, 160) S32, Ho = (H - 1)/2 + 1, Wo = (W - 1)/2 + 1.  Column (ky*7 + kx)*3 + c holds
+ * img[c, 2*oy - 3 + ky, 2*ox - 3 + kx] (0 outside the image); columns 147..159 are 0.  occ_gemm_bf16x3 with the
+ * weight repacked in the same column order then computes the conv. */
+int occ_stem_im2col(const float* img, float* cols, int n, int H, int W, occ_stream_t stream);
+/* ResNet.maxpool = nn.MaxPool2d(3, stride 2, padding 1): in (n, H, W, C) fp32 -> out (n, Ho, Wo, C) S32 with
+ * Ho = (H - 1)/2 + 1, Wo = (W - 1)/2 + 1; padding counts as -inf, a NaN wins as in torch.  C % 32 == 0. */
+int occ_maxpool3x3s2(const float* in, float* out, int n, int H, int W, int C, occ_stream_t stream);
+/* (n, H, W, C) -> (n, H/f, W/f, f*f*C) with column (i*f + j)*C + c = in[f*y + i, f*x + j, c]; f in {2, 4}, H and W
+ * multiples of f, C % 32 == 0.  Whole 32-column chunks are copied unchanged, so S32 stays S32.  With a (Cout, C, f, f)
+ * weight repacked tap-major (occ_conv_bf16x3's layout), a kernel-f stride-f conv becomes a 1x1 conv of the result
+ * (SECONDFPN's deblocks with upsample stride 1/f, second_fpn.py:52-60). */
+int occ_space_to_depth(const float* in, float* out, int n, int H, int W, int C, int f, occ_stream_t stream);
+/* ConvTranspose2d(kernel f, stride f) scatter (SECONDFPN's deblocks with upsample stride f, second_fpn.py:44-51):
+ * in (n*h*w, f*f*C) fp32 = the GEMM of the input rows with the (f*f*C, Cin) matrix whose row (i*f + j)*C + o is
+ * weight[:, o, i, j]; row (b, y, x) column (i*f + j)*C + o goes to pixel (f*y + i, f*x + j), column out_off + o of out
+ * (n*(f*h)*(f*w) rows of ldo floats); the other columns are left untouched.  f in {2, 4}; C, ldo, out_off multiples of 4. */
+int occ_depth_to_space(const float* in, float* out, int n, int h, int w, int C, int f, int ldo, int out_off,
+                       occ_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Dual-path encoder block glue (P/occformer/backbones/dualpath_block.py:65-82).
  * Token rows: voxel tokens ((b*X+x)*Y+y)*Z+z, then BEV tokens B*X*Y*Z + (b*X+x)*Y+y. */
 /* GroupNorm+ReLU of the raw conv output, Z-mean, LayerNorm1 (dualpath_block.py:43-48,69; window_attention.py:355):

@@ -274,7 +274,7 @@ class DepthNet(nn.Module):
         def img(t, c):  # (rows, c) channel-last rows -> the conv's (images, H, W, 1, c) view
             return t.view(n, H, W, 1, c)
 
-        x_s, _ = ops.head_prep(x.float().contiguous().view(n, Cin, HW), False)  # NCHW -> channel-last S32
+        x_s = ops.split_nchw(x.float()).view(n, HW, Cin)  # -> channel-last S32 (no transpose for a channels_last map)
         gates = ops.depthnet_cam_gates(mlp_input.reshape(n, -1).float().contiguous(), *P["gates"])
         xr = ops.conv(img(x_s, Cin), P["reduce"][0], k3, bias=P["reduce"][1], act=1).view(rows, C)
         xd, xd_s, xc_s = ops.se_apply(xr, gates, n, HW)

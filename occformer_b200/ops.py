@@ -394,6 +394,56 @@ def deform_im2col(x_s, off, n, H, W, groups):
     return cols
 
 
+# ----------------------------------------------------------------------------------------------- image encoder
+STEM_COLS = 160  # the 147 (ky, kx, c) columns of the 7x7x3 stem, padded to whole S32 chunks
+
+
+def split_nchw(x):
+    """x (n, C, H, W) fp32 CUDA image map -> its S32 channel-last rows (n, H, W, C), C % 32 == 0.  A channels_last tensor
+    (what this package's image encoder returns) is split in place order by occ_split_rows; any other layout goes through
+    the transposing split of occ_head_prep."""
+    n, C, H, W = x.shape
+    if x.is_contiguous(memory_format=torch.channels_last):
+        return to_split(x.permute(0, 2, 3, 1))
+    return head_prep(x.contiguous().view(n, C, H * W), False)[0].view(n, H, W, C)
+
+
+def stem_im2col(img):
+    """img (n, 3, H, W) fp32 -> S32 columns (n*Ho*Wo, 160) of the 7x7 stride-2 pad-3 stem, column (ky*7 + kx)*3 + c,
+    Ho = (H - 1)//2 + 1 (occ_stem_im2col)."""
+    n, c, H, W = img.shape
+    assert c == 3
+    Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+    cols = torch.empty((n * Ho * Wo, STEM_COLS), dtype=torch.float32, device=img.device)
+    _call("occ_stem_im2col", img, cols, n, H, W)
+    return cols
+
+
+def maxpool3x3s2(x):
+    """x (n, H, W, C) channel-last fp32 -> S32 (n, Ho, Wo, C): nn.MaxPool2d(3, 2, 1) (occ_maxpool3x3s2)."""
+    n, H, W, C = x.shape
+    out = torch.empty((n, (H - 1) // 2 + 1, (W - 1) // 2 + 1, C), dtype=torch.float32, device=x.device)
+    _call("occ_maxpool3x3s2", x, out, n, H, W, C)
+    return out
+
+
+def space_to_depth(x, f):
+    """x (n, H, W, C) -> (n, H/f, W/f, f*f*C), column (i*f + j)*C + c = x[f*y + i, f*x + j, c] (S32 stays S32)."""
+    n, H, W, C = x.shape
+    out = torch.empty((n, H // f, W // f, f * f * C), dtype=torch.float32, device=x.device)
+    _call("occ_space_to_depth", x, out, n, H, W, C, f)
+    return out
+
+
+def depth_to_space_into(x, n, h, w, f, out, out_off):
+    """x (n*h*w, f*f*C) fp32 -> columns [out_off, out_off + C) of out (n*f*h*f*w, ldo), row (b, f*y + i, f*x + j) from
+    column (i*f + j)*C + c of row (b, y, x); the other columns are left as they are.  -> out"""
+    C = x.shape[1] // (f * f)
+    assert x.shape == (n * h * w, f * f * C) and out.dim() == 2 and out.shape[0] == n * h * w * f * f
+    _call("occ_depth_to_space", x, out, n, h, w, C, f, out.shape[1], out_off)
+    return out
+
+
 # ----------------------------------------------------------------------------------------------- encoder glue
 _WL = {}
 

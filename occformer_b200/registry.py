@@ -9,6 +9,9 @@ When mmcv / mmdet / mmdet3d are importable our classes are registered into *thei
 (``force=True`` so that importing this package after the reference plugin swaps the hot-path modules
 in place and the unchanged configs build the H100 versions).  When they are not (this image), a
 minimal local registry with the same ``register_module`` / ``build`` surface is used.
+
+The image encoder's ``ResNet`` and ``SECONDFPN`` are the exception: general mmdet / mmdet3d names, registered in the
+local registries only (``upstream=False``); INTEGRATION.md shows the opt-in.
 """
 
 
@@ -57,10 +60,13 @@ class _Mirror:
             except Exception:
                 pass
 
-    def register_module(self, name=None, force=True, module=None):
+    def register_module(self, name=None, force=True, module=None, upstream=True):
+        """upstream=False registers in the local registry only: for a class whose name is a general mmdet / mmdet3d one
+        (ResNet, SECONDFPN) that must not replace the upstream class for other models in the same process; configs reach
+        it through the local registry or with the class itself as ``type``."""
         def _reg(cls):
             self.local.register_module(name=name, force=True)(cls)
-            for up in self.upstreams:
+            for up in self.upstreams if upstream else ():
                 try:
                     up.register_module(name=name, force=True)(cls)
                 except Exception:

@@ -306,3 +306,79 @@ def make_depthnet_state(cin, mid, ctx, D, cam=27, seed=0):
         else:  # conv / linear weight (out, in, ...): unit gain over the fan-in
             sd[k] = _randn(g, *v.shape, std=v[0].numel() ** -0.5)
     return sd
+
+
+@torch.no_grad()
+def _calibrate_batchnorms(net, inputs, g, jitter=0.05):
+    """Running statistics of every BatchNorm2d of the CPU module ``net`` from one float64 forward on ``inputs``: each
+    BatchNorm gets the batch mean / variance of its own input (variance floored at 1 % of its channel mean, so that no
+    channel that happens to be dead at this size is amplified 300x at another), perturbed slightly (mean + jitter * std *
+    N(0,1), var * (1 + jitter * U(-1,1))).  The statistics are set before each BatchNorm runs, so every layer is
+    calibrated on already calibrated activations.  -> the float32 state_dict"""
+    import torch.nn as nn
+    net = net.double().eval()
+
+    def pre(bn, args):
+        x = args[0]
+        mean, var = x.mean((0, 2, 3)), x.var((0, 2, 3), unbiased=False)
+        var = var + 0.01 * var.mean()
+        bn.running_mean.copy_(mean + jitter * var.sqrt() * _randn(g, *mean.shape).double())
+        bn.running_var.copy_(var * (1 + jitter * (2 * torch.rand(*var.shape, generator=g).double() - 1)))
+
+    hooks = [m.register_forward_pre_hook(pre) for m in net.modules() if isinstance(m, nn.BatchNorm2d)]
+    try:
+        net(*inputs)
+    finally:
+        for h in hooks:
+            h.remove()
+    return {k: (v.float() if v.is_floating_point() else v).clone() for k, v in net.state_dict().items()}
+
+
+def _he_state(net, g):
+    """He-initialised conv weights (std sqrt(2 / fan_in); a ConvTranspose2d's fan-in is its in_channels), BatchNorm
+    weight 1 + 0.1 N(0,1), BatchNorm / conv bias 0.1 N(0,1); running statistics left for calibration"""
+    import torch.nn as nn
+    sd = {}
+    for name, m in net.named_modules():
+        p = name + "." if name else ""
+        if isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)):
+            fan_in = m.weight[0].numel() if isinstance(m, nn.Conv2d) else m.weight.shape[0]
+            sd[p + "weight"] = _randn(g, *m.weight.shape, std=(2.0 / fan_in) ** 0.5)
+            if m.bias is not None:
+                sd[p + "bias"] = 0.1 * _randn(g, *m.bias.shape)
+        elif isinstance(m, nn.BatchNorm2d):
+            sd[p + "weight"] = 1 + 0.1 * _randn(g, m.num_features)
+            sd[p + "bias"] = 0.1 * _randn(g, m.num_features)
+    net.load_state_dict(sd, strict=False)
+    return net
+
+
+def make_resnet_state(seed=0, calib_shape=(4, 3, 64, 96), **resnet_kwargs):
+    """state_dict of image_encoder.ResNet(depth=50, **resnet_kwargs) (mmdet's keys = torchvision resnet50's without fc.*):
+    He-initialised convs, BatchNorm affine 1 + 0.1 N / 0.1 N, and running statistics calibrated on a seeded fp64 forward
+    of N(0,1) images of calib_shape (then perturbed slightly), so that the 16 stacked blocks neither vanish nor blow up
+    on images of that kind at any size.  No BatchNorm weight is zero.
+
+    The last BatchNorm of each residual branch (bn3) has weight 0.25 (1 + 0.1 N): the branch is smaller than the identity
+    path, as in trained ResNets.  With bn3 weights around 1 the random stack is chaotic: a relative perturbation of 1e-5
+    of every conv weight grows to 3e-3 at layer4 (fp64 on the host), so no fp32 implementation, cuDNN's included, could
+    be compared with another at the 1e-3 gate."""
+    from .image_encoder import ResNet
+    g = torch.Generator().manual_seed(seed)
+    net = _he_state(ResNet(depth=50, **resnet_kwargs), g)
+    with torch.no_grad():
+        for name, m in net.named_modules():
+            if name.endswith(".bn3"):
+                m.weight.mul_(0.25)
+    return _calibrate_batchnorms(net, [_randn(g, *calib_shape).double()], g)
+
+
+def make_secondfpn_state(in_channels, out_channels, upsample_strides, seed=0, out_hw=(4, 8), n=2, **fpn_kwargs):
+    """state_dict of image_encoder.SECONDFPN(in_channels, out_channels, upsample_strides, **fpn_kwargs) (the reference's
+    deblocks.{i}.{0,1}.* keys): He-initialised (de)convs, BatchNorm affine 1 + 0.1 N / 0.1 N, running statistics
+    calibrated on seeded non-negative (post-ReLU-like) levels |N(0,1)| whose sizes map to out_hw."""
+    from .image_encoder import SECONDFPN
+    g = torch.Generator().manual_seed(seed)
+    net = _he_state(SECONDFPN(in_channels, out_channels, upsample_strides, **fpn_kwargs), g)
+    levels = [_randn(g, n, c, int(out_hw[0] / s), int(out_hw[1] / s)).abs() for c, s in zip(in_channels, upsample_strides)]
+    return _calibrate_batchnorms(net, [[t.double() for t in levels]], g)
