@@ -98,7 +98,8 @@ int occ_bev_pool(const float* feats, const long long* coords, float* out, int n,
  *   MSDeformAttnPixelDecoder3D  P/occformer/necks/multiscale_deformattn_3d.py:60-141 (input/lateral/output convs, Linears)
  *   Mask2Former*OccHead       P/occformer/mask2former/mask2former_nusc_occ.py:446-457 (mask einsum), decoder K/V proj
  * out[M,N] = act(A[M,K] W[N,K]^T + bias + residual): the residual is added BEFORE the activation (ResNet's
- * relu(bn2(conv2) + identity)); A, W in S32 (K % 32 == 0); act: 0 none, 1 ReLU, 2 GELU(erf); split_out: write out in
+ * relu(bn2(conv2) + identity)); A, W in S32 (K % 32 == 0); act: 0 none, 1 ReLU, 2 GELU(erf), 3 Swish x*sigmoid(x)
+ * (mmcv Swish); split_out: write out in
  * S32 (N % 32 == 0) instead of fp32; bias / residual fp32. */
 int occ_gemm_bf16x3(const float* A, const float* W, float* out, int M, int N, int K, const float* bias,
                     const float* residual, int act, int split_out, occ_stream_t stream);
@@ -180,11 +181,15 @@ int occ_deform_im2col(const float* x, const float* off, int off_ld, float* cols,
  * (M/models/necks/second_fpn.py:11-91), inference with eval-mode BatchNorms folded into the convolutions.  Every
  * convolution is an occ_gemm_bf16x3 / occ_conv_bf16x3 / occ_conv_slice_bf16x3 launch; the entry points below are the
  * layout steps those cannot do.  Activations are channel-last rows (image, y, x) of C floats. */
-/* ResNet stem conv1 (7x7, stride 2, padding 3, Cin = 3; ResNet._make_stem_layer) as im2col: img (n, 3, H, W) NCHW fp32
- * -> cols (n*Ho*Wo, 160) S32, Ho = (H - 1)/2 + 1, Wo = (W - 1)/2 + 1.  Column (ky*7 + kx)*3 + c holds
- * img[c, 2*oy - 3 + ky, 2*ox - 3 + kx] (0 outside the image); columns 147..159 are 0.  occ_gemm_bf16x3 with the
- * weight repacked in the same column order then computes the conv. */
-int occ_stem_im2col(const float* img, float* cols, int n, int H, int W, occ_stream_t stream);
+/* A stem conv on Cin = 3 as im2col: img (n, 3, H, W) NCHW fp32 -> cols (n*Ho*Wo, ncols) S32.  Column (ky*k + kx)*3 + c
+ * holds img[c, stride*oy - pad_top + ky, stride*ox - pad_left + kx] (0 outside the image); columns 3*k*k .. ncols-1 are
+ * 0 (ncols % 32 == 0).  The caller gives the output size, so the bottom / right padding is whatever Ho, Wo imply.
+ * occ_gemm_bf16x3 with the weight repacked in the same column order then computes the conv.
+ *   ResNet conv1 (ResNet._make_stem_layer): k 7, stride 2, pads 3 / 3, Ho = (H - 1)/2 + 1, ncols 160.
+ *   CustomEfficientNet layers.0 (P/occformer/backbones/efficientnet.py:418-427, mmcv Conv2dAdaptivePadding): k 3,
+ *   stride 2, Ho = ceil(H/2), top / left pad = pad // 2 of pad = max((Ho - 1)*2 + 3 - H, 0), ncols 32. */
+int occ_stem_im2col(const float* img, float* cols, int n, int H, int W, int k, int stride, int pad_top, int pad_left,
+                    int Ho, int Wo, int ncols, occ_stream_t stream);
 /* ResNet.maxpool = nn.MaxPool2d(3, stride 2, padding 1): in (n, H, W, C) fp32 -> out (n, Ho, Wo, C) S32 with
  * Ho = (H - 1)/2 + 1, Wo = (W - 1)/2 + 1; padding counts as -inf, a NaN wins as in torch.  C % 32 == 0. */
 int occ_maxpool3x3s2(const float* in, float* out, int n, int H, int W, int C, occ_stream_t stream);
@@ -199,6 +204,33 @@ int occ_space_to_depth(const float* in, float* out, int n, int H, int W, int C, 
  * (n*(f*h)*(f*w) rows of ldo floats); the other columns are left untouched.  f in {2, 4}; C, ldo, out_off multiples of 4. */
 int occ_depth_to_space(const float* in, float* out, int n, int h, int w, int C, int f, int ldo, int out_off,
                        occ_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
+ * EfficientNet image encoder of the SemanticKITTI model (projects/configs/occformer_kitti/occformer_kitti.py:66-80,
+ * img_backbone = CustomEfficientNet(arch='b7'), P/occformer/backbones/efficientnet.py).  Per InvertedResidual block
+ * (:204-222): expand conv = occ_gemm_bf16x3 act 3 (Swish), the depthwise conv below, occ_se_gate, occ_se_scale, linear
+ * conv = occ_gemm_bf16x3 with the residual.  Activations are channel-last rows (image, y, x) of C floats with C a multiple
+ * of 32; a narrower layer is zero-padded (zero weights, biases and BatchNorm entries), so its pad channels stay 0. */
+/* Number of per-CTA SE partial sums occ_dwconv_swish writes per image and channel for an Ho x Wo output. */
+int occ_dw_tiles(int Ho, int Wo);
+/* Depthwise conv + folded BatchNorm + Swish (the depthwise_conv ConvModule, :180-189, groups = C, mmcv
+ * Conv2dAdaptivePadding): in (n, H, W, C) fp32 -> out (n, Ho, Wo, C) fp32,
+ *   out[o, c] = swish(bias[c] + sum over (ky, kx) in order of w[ky*k + kx, c] * in[stride*oy - pad_top + ky,
+ *                                                                              stride*ox - pad_left + kx, c])
+ * with taps outside the input skipped (zero padding; the bottom / right padding is what Ho, Wo imply).  w tap-major
+ * (k*k, C), bias (C); k in {3, 5}, stride in {1, 2}, C % 32 == 0, n <= 65535, all pointers 16-byte aligned.
+ * The same launch writes partials (n, occ_dw_tiles(Ho, Wo), C): per-CTA sums of out over its pixels, in a fixed order
+ * (bit-reproducible; occ_se_gate reduces them). */
+int occ_dwconv_swish(const float* in, const float* w, const float* bias, float* out, float* partials, int n, int H, int W,
+                     int C, int k, int stride, int pad_top, int pad_left, int Ho, int Wo, occ_stream_t stream);
+/* mmdet 2.14 SELayer(C, ratio, act_cfg=(Swish, Sigmoid)) gate, fp32, one CTA per image: mean[c] = (sum over the tiles in
+ * order of partials[img, t, c]) / hw, s = swish(W1 mean + b1), gate[img] = sigmoid(W2 s + b2).  Weights K-major:
+ * w1T (C, S), b1 (S), w2T (S, C), b2 (C); gate (n, C).  C <= 8192, S <= 512. */
+int occ_se_gate(const float* partials, int tiles, int hw, const float* w1T, const float* b1, const float* w2T,
+                const float* b2, float* gate, int n, int C, int S, occ_stream_t stream);
+/* SELayer output x * gate (:214-215) as the linear conv's operand: y (n*rows_per_img, C) fp32, gate (n, C) -> out S32;
+ * C % 32 == 0, pointers 16-byte aligned. */
+int occ_se_scale(const float* y, const float* gate, float* out, int n, int rows_per_img, int C, occ_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Dual-path encoder block glue (P/occformer/backbones/dualpath_block.py:65-82).

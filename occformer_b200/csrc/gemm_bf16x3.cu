@@ -45,7 +45,7 @@ struct GemmParams {
   int ldr;
   int splits;     // split-K: > 1 => every tile's k-blocks are divided among `splits` CTAs, partial sums meet in `out`
                   // (zero-initialised by the host) through TMA reduce-add; no bias / act / stats in the kernel
-  int act;        // 0 none, 1 relu, 2 gelu(erf)
+  int act;        // 0 none, 1 relu, 2 gelu(erf), 3 swish
   int split_out;  // write the result in the S32 split format (the consumer is another tensor-core contraction)
   int passes;     // tensor-core passes per 32-k block (occ_common.cuh: mma_passes)
   // conv mode
@@ -72,6 +72,8 @@ struct GemmParams {
 constexpr int SPLITK_SEMS = 1024;
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
+// mmcv Swish (x * sigmoid(x)), the activation of EfficientNet's convs
+__device__ __forceinline__ float swish(float x) { return x / (1.0f + expf(-x)); }
 
 template <int CPG>
 __device__ __forceinline__ void accum_stats(const float (&v)[32], float (&sv)[32]) {
@@ -441,6 +443,9 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         } else if (p.act == 2) {
 #pragma unroll
           for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
+        } else if (p.act == 3) {
+#pragma unroll
+          for (int j = 0; j < 32; ++j) v[j] = swish(v[j]);
         }
         if (p.split_out) {  // the 32 values of this (row, chunk) become the 32 words of their S32 chunk
           uint32_t w[32];
@@ -691,7 +696,7 @@ extern "C" int occ_gemm_bf16x3(const float* A, const float* W, float* out, int M
   OCC_REQUIRE(K % 32 == 0);                 // S32 operand rows: whole 32-k chunks
   OCC_REQUIRE(!split_out || N % 32 == 0);   // S32 output rows
   OCC_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(W) & 15) == 0);
-  OCC_REQUIRE(act >= 0 && act <= 2);
+  OCC_REQUIRE(act >= 0 && act <= 3);
   GemmParams p{};
   p.passes = mma_passes();
   p.M = M; p.N = N; p.K = K; p.num_k_blocks = (K + BK - 1) / BK;
@@ -734,7 +739,7 @@ static int conv_bf16x3(const float* x, const float* w2, float* out, int ldo, int
   OCC_REQUIRE(Cin % BK == 0);
   OCC_REQUIRE((KX == 1 || KX == 3) && (KY == 1 || KY == 3) && (KZ == 1 || KZ == 3));
   OCC_REQUIRE(stride == 1 || stride == 2);
-  OCC_REQUIRE(dil >= 1 && act >= 0 && act <= 2);
+  OCC_REQUIRE(dil >= 1 && act >= 0 && act <= 3);
   OCC_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(w2) & 15) == 0);
   if (gn_stats) OCC_REQUIRE(cpg >= 1 && Cout % cpg == 0 && Cout / cpg <= MAX_STAT_GROUPS);
   GemmParams p{};

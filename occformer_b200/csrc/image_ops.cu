@@ -1,5 +1,6 @@
 // The layout kernels of the image encoder (mmdet ResNet-50 + mmdet3d SECONDFPN, the img_backbone / img_neck of the
-// nuScenes R50 model) that the convolutions cannot do themselves: the stem's im2col (Cin = 3, 7x7), the stem max-pool,
+// nuScenes R50 model; EfficientNet's stem) that the convolutions cannot do themselves: the stem's im2col (Cin = 3, any
+// k x k, stride and top / left padding), the stem max-pool,
 // and the pixel reshuffles that turn SECONDFPN's stride-f convs and transposed convs into 1x1 convs / GEMMs.  Every
 // contraction of the encoder goes through occ_gemm_bf16x3 / occ_conv_bf16x3 / occ_conv_slice_bf16x3; activations are
 // channel-last rows (image, y, x).
@@ -10,27 +11,26 @@
 
 namespace occ {
 
-constexpr int STEM_K = 7 * 7 * 3;  // 147 taps x channels, padded to STEM_COLS (whole S32 chunks)
-constexpr int STEM_COLS = 160;
-
-// One warp per output pixel; lane l owns column l of each of the five 32-column chunks and writes its hi / lo bf16 halves
-// (every chunk is one coalesced 128-byte store).  Column k < 147: (ky, kx, c) = (k / 21, k / 3 % 7, k % 3).
+// One warp per output pixel; lane l owns column l of each 32-column chunk and writes its hi / lo bf16 halves (every
+// chunk is one coalesced 128-byte store).  Column q < 3*k*k: (ky, kx, c) = (q / (3k), q / 3 % k, q % 3), input pixel
+// (stride*oy - pad_top + ky, stride*ox - pad_left + kx); columns >= 3*k*k and pixels outside the image are 0.
 __global__ void __launch_bounds__(256)
-stem_im2col_kernel(const float* __restrict__ img, float* __restrict__ cols, long long rows, int H, int W, int Ho, int Wo) {
+stem_im2col_kernel(const float* __restrict__ img, float* __restrict__ cols, long long rows, int H, int W, int Ho, int Wo,
+                   int k, int stride, int pad_top, int pad_left, int ncols) {
   const long long r = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (r >= rows) return;
   const long long b = r / ((long long)Ho * Wo);
   const int pix = (int)(r - b * Ho * Wo);
   const int oy = pix / Wo, ox = pix - (pix / Wo) * Wo;
-  __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(cols + r * STEM_COLS);
-#pragma unroll
-  for (int q = 0; q < STEM_COLS / 32; ++q) {
-    const int k = q * 32 + lane;
+  const int taps3 = 3 * k * k;
+  __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(cols + r * ncols);
+  for (int q = 0; q < ncols / 32; ++q) {
+    const int col = q * 32 + lane;
     float v = 0.f;
-    if (k < STEM_K) {
-      const int c = k % 3, t = k / 3;
-      const int iy = 2 * oy - 3 + t / 7, ix = 2 * ox - 3 + t % 7;
+    if (col < taps3) {
+      const int c = col % 3, t = col / 3;
+      const int iy = stride * oy - pad_top + t / k, ix = stride * ox - pad_left + t % k;
       if (iy >= 0 && iy < H && ix >= 0 && ix < W) v = __ldg(img + ((b * 3 + c) * H + iy) * W + ix);
     }
     const __nv_bfloat16 hi = __float2bfloat16_rn(v);
@@ -109,12 +109,15 @@ static unsigned blocks_of(long long threads) { return (unsigned)((threads + 255)
 
 using namespace occ;
 
-extern "C" int occ_stem_im2col(const float* img, float* cols, int n, int H, int W, cudaStream_t stream) {
-  OCC_REQUIRE(img && cols && n > 0 && H > 0 && W > 0 && aligned16(cols));
-  const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
+extern "C" int occ_stem_im2col(const float* img, float* cols, int n, int H, int W, int k, int stride, int pad_top,
+                               int pad_left, int Ho, int Wo, int ncols, cudaStream_t stream) {
+  OCC_REQUIRE(img && cols && n > 0 && H > 0 && W > 0 && Ho > 0 && Wo > 0 && aligned16(cols));
+  OCC_REQUIRE(k >= 1 && k <= 7 && stride >= 1 && pad_top >= 0 && pad_left >= 0 && pad_top < k && pad_left < k);
+  OCC_REQUIRE(ncols % 32 == 0 && ncols >= 3 * k * k);
   const long long rows = (long long)n * Ho * Wo;
   OCC_REQUIRE((rows + 7) / 8 < (1ll << 31));
-  stem_im2col_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(img, cols, rows, H, W, Ho, Wo);
+  stem_im2col_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(img, cols, rows, H, W, Ho, Wo, k, stride, pad_top,
+                                                                      pad_left, ncols);
   OCC_LAUNCH_CHECK();
   return OCC_OK;
 }

@@ -260,11 +260,26 @@ class ResNet(_Prepared):
 
 
 # ---------------------------------------------------------------------------------------------------------- SECONDFPN
+def _round32(c):
+    return (c + 31) // 32 * 32
+
+
+def _twin(t):
+    """the S32 twin (n, H, W, round_up(C, 32)) a backbone stage carries as ``_occ_s32`` (zero pad columns when C is not
+    a multiple of 32), or None"""
+    n, C, H, W = t.shape
+    t_s = getattr(t, "_occ_s32", None)
+    if t_s is None or t_s.shape != (n, H, W, _round32(C)) or t_s.device != t.device:
+        return None
+    return t_s
+
+
 @NECKS.register_module(upstream=False)
 class SECONDFPN(_Prepared):
     """second_fpn.py:11-91: one deblock per level -- ConvTranspose2d(kernel = stride = s) for an upsample stride s >= 1
     (s == 1 also Conv2d(1x1) with use_conv_for_no_stride), Conv2d(kernel = stride = 1/s) for s < 1 -- each followed by
-    BatchNorm (default eps 1e-3) and ReLU; forward(levels) -> [channel concat of the deblock outputs]."""
+    BatchNorm (default eps 1e-3) and ReLU; forward(levels) -> [channel concat of the deblock outputs].  On CUDA a level
+    whose width is not a multiple of 32 must carry its zero-padded S32 twin (CustomEfficientNet's stages do)."""
 
     def __init__(self, in_channels=[128, 128, 256], out_channels=[256, 256, 256], upsample_strides=[1, 2, 4],
                  norm_cfg=dict(type="BN", eps=1e-3, momentum=0.01), upsample_cfg=dict(type="deconv", bias=False),
@@ -317,13 +332,15 @@ class SECONDFPN(_Prepared):
         conv of the space_to_depth'd input; a stride-f deconv as the S32 (f*f*Cout, Cin) matrix whose row (i*f + j)*Cout
         + o is w[:, o, i, j], with its bias repeated per (i, j).  Cached; a load_state_dict or .to() drops the cache."""
         P = []
-        for kind, f, w, b in self._folded():
+        for (kind, f, w, b), cin in zip(self._folded(), self.in_channels):
+            pad = _round32(cin) - cin  # zero input columns (per tap) for a level whose S32 twin is zero-padded
             if kind == "conv":
-                P.append(("down", f, ops.repack_conv_weight(w)[0], b))
+                P.append(("down", f, ops.repack_conv_weight(F.pad(w, (0, 0, 0, 0, 0, pad)))[0], b))
             elif f == 1:
-                P.append(("down", 1, ops.split_weight(w[:, :, 0, 0].t()), b))
+                P.append(("down", 1, ops.split_weight(F.pad(w[:, :, 0, 0].t(), (0, pad))), b))
             else:
-                P.append(("up", f, ops.split_weight(w.permute(2, 3, 1, 0).reshape(-1, w.shape[0])), b.repeat(f * f)))
+                P.append(("up", f, ops.split_weight(F.pad(w.permute(2, 3, 1, 0).reshape(-1, w.shape[0]), (0, pad))),
+                          b.repeat(f * f)))
         self._prep = P
         return P
 
@@ -338,8 +355,10 @@ class SECONDFPN(_Prepared):
         need = []
         if any(t.dim() != 4 or t.shape[1] != c for t, c in zip(x, self.in_channels)):
             need.append(f"levels of shape (n, C_i, H_i, W_i) with C_i = {self.in_channels}")
-        if any(c % 32 for c in self.in_channels + self.out_channels):
-            need.append("in_channels and out_channels multiples of 32 (whole 32-channel chunks)")
+        if any(c % 32 for c in self.out_channels) or (not need and any(
+                c % 32 and _twin(t) is None for t, c in zip(x, self.in_channels))):
+            need.append("in_channels and out_channels multiples of 32 (whole 32-channel chunks; a narrower level must "
+                        "carry its S32 twin zero-padded to whole chunks, as CustomEfficientNet hands it over)")
         if any(s not in (0.25, 0.5, 1, 2, 4) for s in self.upsample_strides):
             need.append("upsample_strides in {0.25, 0.5, 1, 2, 4}")
         if not need:
@@ -366,9 +385,10 @@ class SECONDFPN(_Prepared):
         off = 0
         for t, (kind, f, w, b), cout in zip(x, P, self.out_channels):
             _, C, H, W = t.shape
-            t_s = getattr(t, "_occ_s32", None)
-            if t_s is None or t_s.shape != (n, H, W, C) or t_s.device != t.device:
+            t_s = _twin(t)
+            if t_s is None:
                 t_s = ops.split_nchw(t.float())
+            C = t_s.shape[-1]
             if kind == "down":
                 if f > 1:
                     t_s = ops.space_to_depth(t_s, f)

@@ -277,7 +277,8 @@ def bev_pool_channel_last(feats, coords, B, X, Y, Z, return_workspace=False):
 
 # ----------------------------------------------------------------------------------------------- GEMM / conv
 def gemm(a, w, bias=None, residual=None, act=0, split_out=False, out=None):
-    """out[M,N] = act(a[M,K] @ w[N,K]^T + bias + residual): the residual is added before the activation.  a, w in S32
+    """out[M,N] = act(a[M,K] @ w[N,K]^T + bias + residual), act 0 none, 1 ReLU, 2 GELU, 3 Swish: the residual is added
+    before the activation.  a, w in S32
     (to_split / split_weight / a producer's split output); out fp32, or S32 when split_out (operand of the next
     contraction)."""
     M, K = a.shape
@@ -412,10 +413,17 @@ def stem_im2col(img):
     """img (n, 3, H, W) fp32 -> S32 columns (n*Ho*Wo, 160) of the 7x7 stride-2 pad-3 stem, column (ky*7 + kx)*3 + c,
     Ho = (H - 1)//2 + 1 (occ_stem_im2col)."""
     n, c, H, W = img.shape
-    assert c == 3
-    Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
-    cols = torch.empty((n * Ho * Wo, STEM_COLS), dtype=torch.float32, device=img.device)
-    _call("occ_stem_im2col", img, cols, n, H, W)
+    return im2col3(img, 7, 2, 3, 3, (H - 1) // 2 + 1, (W - 1) // 2 + 1, STEM_COLS)
+
+
+def im2col3(img, k, stride, pad_top, pad_left, Ho, Wo, ncols):
+    """img (n, 3, H, W) fp32 -> S32 columns (n*Ho*Wo, ncols) of a k x k conv on 3 channels: column (ky*k + kx)*3 + c =
+    img[c, stride*oy - pad_top + ky, stride*ox - pad_left + kx], 0 outside the image and in columns >= 3*k*k
+    (occ_stem_im2col)."""
+    n, c, H, W = img.shape
+    assert c == 3 and ncols % 32 == 0 and ncols >= 3 * k * k
+    cols = torch.empty((n * Ho * Wo, ncols), dtype=torch.float32, device=img.device)
+    _call("occ_stem_im2col", img, cols, n, H, W, k, stride, pad_top, pad_left, Ho, Wo, ncols)
     return cols
 
 
@@ -441,6 +449,36 @@ def depth_to_space_into(x, n, h, w, f, out, out_off):
     C = x.shape[1] // (f * f)
     assert x.shape == (n * h * w, f * f * C) and out.dim() == 2 and out.shape[0] == n * h * w * f * f
     _call("occ_depth_to_space", x, out, n, h, w, C, f, out.shape[1], out_off)
+    return out
+
+
+# ----------------------------------------------------------------------------------------------- EfficientNet block
+def dwconv_swish(x, w, b, k, stride, pad_top, pad_left, Ho, Wo):
+    """Depthwise k x k conv + folded BatchNorm + Swish: x (n, H, W, C) fp32, w (k*k, C) tap-major, b (C) -> (out (n, Ho,
+    Wo, C) fp32, SE partial sums (n, tiles, C)) (occ_dwconv_swish)."""
+    n, H, W, C = x.shape
+    tiles = lib().occ_dw_tiles(Ho, Wo)
+    out = torch.empty((n, Ho, Wo, C), dtype=torch.float32, device=x.device)
+    part = torch.empty((n, tiles, C), dtype=torch.float32, device=x.device)
+    _call("occ_dwconv_swish", x, w, b, out, part, n, H, W, C, k, stride, pad_top, pad_left, Ho, Wo)
+    return out, part
+
+
+def se_gate(part, hw, w1T, b1, w2T, b2):
+    """SELayer gate from occ_dwconv_swish's partial sums (n, tiles, C) of an hw-pixel map: w1T (C, S), b1 (S), w2T (S, C),
+    b2 (C) -> gate (n, C) = sigmoid(W2 swish(W1 mean + b1) + b2) (occ_se_gate)."""
+    n, tiles, C = part.shape
+    S = b1.shape[0]
+    gate = torch.empty((n, C), dtype=torch.float32, device=part.device)
+    _call("occ_se_gate", part, tiles, hw, w1T, b1, w2T, b2, gate, n, C, S)
+    return gate
+
+
+def se_scale(y, gate):
+    """y (n, ..., C) fp32, gate (n, C) -> y * gate[image] in S32, same shape (occ_se_scale)."""
+    n, C = gate.shape
+    out = torch.empty_like(y)
+    _call("occ_se_scale", y, gate, out, n, y.numel() // (n * C), C)
     return out
 
 

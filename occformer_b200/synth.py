@@ -309,11 +309,11 @@ def make_depthnet_state(cin, mid, ctx, D, cam=27, seed=0):
 
 
 @torch.no_grad()
-def _calibrate_batchnorms(net, inputs, g, jitter=0.05):
+def _calibrate_batchnorms(net, inputs, g, jitter=0.05, floor=0.01):
     """Running statistics of every BatchNorm2d of the CPU module ``net`` from one float64 forward on ``inputs``: each
-    BatchNorm gets the batch mean / variance of its own input (variance floored at 1 % of its channel mean, so that no
-    channel that happens to be dead at this size is amplified 300x at another), perturbed slightly (mean + jitter * std *
-    N(0,1), var * (1 + jitter * U(-1,1))).  The statistics are set before each BatchNorm runs, so every layer is
+    BatchNorm gets the batch mean / variance of its own input (variance floored at ``floor`` (1 %) of its channel mean, so
+    that no channel that happens to be dead at this size is amplified 300x at another), perturbed slightly (mean + jitter *
+    std * N(0,1), var * (1 + jitter * U(-1,1))).  The statistics are set before each BatchNorm runs, so every layer is
     calibrated on already calibrated activations.  -> the float32 state_dict"""
     import torch.nn as nn
     net = net.double().eval()
@@ -321,7 +321,7 @@ def _calibrate_batchnorms(net, inputs, g, jitter=0.05):
     def pre(bn, args):
         x = args[0]
         mean, var = x.mean((0, 2, 3)), x.var((0, 2, 3), unbiased=False)
-        var = var + 0.01 * var.mean()
+        var = var + floor * var.mean()
         bn.running_mean.copy_(mean + jitter * var.sqrt() * _randn(g, *mean.shape).double())
         bn.running_var.copy_(var * (1 + jitter * (2 * torch.rand(*var.shape, generator=g).double() - 1)))
 
@@ -382,3 +382,32 @@ def make_secondfpn_state(in_channels, out_channels, upsample_strides, seed=0, ou
     net = _he_state(SECONDFPN(in_channels, out_channels, upsample_strides, **fpn_kwargs), g)
     levels = [_randn(g, n, c, int(out_hw[0] / s), int(out_hw[1] / s)).abs() for c, s in zip(in_channels, upsample_strides)]
     return _calibrate_batchnorms(net, [[t.double() for t in levels]], g)
+
+
+def make_efficientnet_state(arch="b7", seed=0, calib_shape=(1, 3, 384, 1280), linear_bn_gain=0.25, floor=16.0, **kwargs):
+    """state_dict of efficientnet.CustomEfficientNet(arch, **kwargs) (the reference's keys): He-initialised convs (the
+    SE convs too, with bias 0.1 N), BatchNorm affine 1 + 0.1 N / 0.1 N, and running statistics calibrated on a seeded fp64
+    forward of N(0,1) images of calib_shape (then perturbed slightly), so that the stacked blocks neither vanish nor blow
+    up on images of that size.
+
+    Three things keep B7's 55 random blocks from being chaotic (measured in fp64 on the host as the growth of a 1e-5
+    relative perturbation of every conv / BatchNorm weight; at 1e-3 or more no two fp32 implementations could be compared
+    at the 1e-3 gate):
+    - each block's last BatchNorm (linear_conv.bn, before the residual add) has weight linear_bn_gain * (1 + 0.1 N), as
+      ResNet's bn3 in make_resnet_state: the branch is smaller than the identity path, as in trained networks;
+    - the calibrated variances are floored at ``floor`` = 16x the layer's mean channel variance (make_resnet_state:
+      1 %), so that no near-constant channel is lifted 10x; every BatchNorm then scales its channels down about 4x, and
+      the Swish after it works near its linear part;
+    - the calibration images have the KITTI size.  Calibrated at 96x320, layers.5 sees 3x10 maps on which most 5x5
+      depthwise taps fall into the padding; at 384x1280 its interior pixels then have a larger variance than calibrated.
+    Measured at (1, 3, 384, 1280), calibrated there: the perturbation reaches 2.1e-4 at layers.6 (floor 4x: 5.2e-4; 1 %
+    floor and calibration at 96x320: 0.43 already at 192x640).
+    About half of every stage's activations are positive."""
+    from .efficientnet import CustomEfficientNet
+    g = torch.Generator().manual_seed(seed)
+    net = _he_state(CustomEfficientNet(arch=arch, **kwargs), g)
+    with torch.no_grad():
+        for name, m in net.named_modules():
+            if name.endswith("linear_conv.bn"):
+                m.weight.mul_(linear_bn_gain)
+    return _calibrate_batchnorms(net, [_randn(g, *calib_shape).double()], g, floor=floor)
