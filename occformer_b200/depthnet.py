@@ -22,6 +22,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import ops
+from .common import PreparedModule, fold_bn
 
 
 class BasicBlock(nn.Module):
@@ -134,7 +135,7 @@ class DCN(nn.Module):
         return torch.einsum("bgckhw,gock->bgohw", col, w).reshape(B, -1, H, W)
 
 
-class DepthNet(nn.Module):
+class DepthNet(PreparedModule):
     """ViewTransformerLSSBEVDepth.py:450-504: camera-aware depth / context heads.  forward(x (B*N, Cin, fH, fW),
     mlp_input (B, N, cam_channels)) -> (B*N, D + C_ctx, fH, fW) = depth logits | context features."""
 
@@ -154,15 +155,6 @@ class DepthNet(nn.Module):
                                         BasicBlock(mid_channels, mid_channels), ASPP(mid_channels, mid_channels),
                                         DCN(mid_channels, mid_channels, 3, padding=1, groups=4),
                                         nn.Conv2d(mid_channels, depth_channels, 1))
-        self._prep = None
-        self.register_load_state_dict_post_hook(lambda m, k: m._invalidate())
-
-    def _invalidate(self):
-        self._prep = None
-
-    def _apply(self, fn, *a, **k):
-        self._prep = None
-        return super()._apply(fn, *a, **k)
 
     def forward(self, x, mlp_input):
         """x (B*N, Cin, fH, fW), mlp_input (B, N, cam_channels) -> (B*N, D + C_ctx, fH, fW)."""
@@ -173,21 +165,14 @@ class DepthNet(nn.Module):
     # ------------------------------------------------------------------ parameters of the CUDA forward
     @torch.no_grad()
     def _folded(self):
-        """Eval-mode BatchNorms folded into the layer before them, in fp64, rounded to fp32 (natural layouts, on the
-        parameters' device): w' = w * g / sqrt(var + eps), b' = (b - mean) * g / sqrt(var + eps) + beta.  Also the
-        BatchNorm1d of mlp_input folded into both fc1's, conv_offset padded to 32 output channels and the DCN weight as
-        `groups` tap-major matrices (Cout/groups, 9 * Cin/groups), column k * Cin/groups + c."""
-        def fold(w, b, bn):
-            s = bn.weight.double() / torch.sqrt(bn.running_var.double() + bn.eps)
-            b0 = b.double() if b is not None else torch.zeros_like(s)
-            w = w.double() * s.view(-1, *([1] * (w.dim() - 1)))
-            return w.float().contiguous(), ((b0 - bn.running_mean.double()) * s + bn.bias.double()).float().contiguous()
-
+        """Eval-mode BatchNorms folded into the layer before them (common.fold_bn; natural layouts, on the parameters'
+        device).  Also the BatchNorm1d of mlp_input folded into both fc1's, conv_offset padded to 32 output channels and
+        the DCN weight as `groups` tap-major matrices (Cout/groups, 9 * Cin/groups), column k * Cin/groups + c."""
         def plain(layer):
             return layer.weight.detach().float().contiguous(), layer.bias.detach().float().contiguous()
 
         F_ = {}
-        F_["reduce"] = fold(self.reduce_conv[0].weight, self.reduce_conv[0].bias, self.reduce_conv[1])
+        F_["reduce"] = fold_bn(self.reduce_conv[0].weight, self.reduce_conv[0].bias, self.reduce_conv[1])
         F_["ctx"] = plain(self.context_conv)
         s = self.bn.weight.double() / torch.sqrt(self.bn.running_var.double() + self.bn.eps)
         t = self.bn.bias.double() - self.bn.running_mean.double() * s  # bn(m) = s * m + t
@@ -198,13 +183,14 @@ class DepthNet(nn.Module):
                           *plain(mlp.fc2), se.conv_reduce.weight.detach().float()[:, :, 0, 0], se.conv_reduce.bias.detach().float(),
                           se.conv_expand.weight.detach().float()[:, :, 0, 0], se.conv_expand.bias.detach().float()))
         F_["gates"] = tuple(torch.stack([a, b]).contiguous() for a, b in zip(*gates))  # (2, ...) depth | context
-        F_["blocks"] = [fold(blk.conv1.weight, None, blk.bn1) + fold(blk.conv2.weight, None, blk.bn2)
+        F_["blocks"] = [fold_bn(blk.conv1.weight, None, blk.bn1) + fold_bn(blk.conv2.weight, None, blk.bn2)
                         for blk in self.depth_conv[:3]]
         aspp = self.depth_conv[3]
-        F_["aspp"] = [fold(m.atrous_conv.weight, None, m.bn) for m in (aspp.aspp1, aspp.aspp2, aspp.aspp3, aspp.aspp4)]
-        gw, gb = fold(aspp.global_avg_pool[1].weight, None, aspp.global_avg_pool[2])
+        F_["aspp"] = [fold_bn(m.atrous_conv.weight, None, m.bn)
+                      for m in (aspp.aspp1, aspp.aspp2, aspp.aspp3, aspp.aspp4)]
+        gw, gb = fold_bn(aspp.global_avg_pool[1].weight, None, aspp.global_avg_pool[2])
         F_["gap"] = (gw[:, :, 0, 0].contiguous(), gb)
-        F_["aspp_c1"] = fold(aspp.conv1.weight, None, aspp.bn1)
+        F_["aspp_c1"] = fold_bn(aspp.conv1.weight, None, aspp.bn1)
         dcn = self.depth_conv[4]
         ow, ob = plain(dcn.conv_offset)
         F_["offset"] = (torch.cat([ow, ow.new_zeros(32 - ow.shape[0], *ow.shape[1:])]).contiguous(),
@@ -219,7 +205,7 @@ class DepthNet(nn.Module):
     @torch.no_grad()
     def _prepare(self):
         """The folded parameters in the kernels' layouts: conv weights repacked tap-major in S32, the gate weights
-        K-major (in, out), the DCN group matrices in S32.  Cached; a load_state_dict or .to() drops the cache."""
+        K-major (in, out), the DCN group matrices in S32."""
         F_ = self._folded()
         P = {}
         P["reduce"] = (ops.repack_conv_weight(F_["reduce"][0])[0], F_["reduce"][1])
@@ -234,7 +220,6 @@ class DepthNet(nn.Module):
         P["offset"] = (ops.repack_conv_weight(F_["offset"][0])[0], F_["offset"][1])
         P["dcn"] = [ops.split_weight(m) for m in F_["dcn"]]
         P["depth"] = (ops.repack_conv_weight(F_["depth"][0])[0], F_["depth"][1])
-        self._prep = P
         return P
 
     def _check_cuda_contract(self, x, mlp_input):
@@ -265,7 +250,7 @@ class DepthNet(nn.Module):
     @torch.no_grad()
     def _forward_cuda(self, x, mlp_input):
         self._check_cuda_contract(x, mlp_input)
-        P = self._prep or self._prepare()
+        P = self.prepared()
         n, Cin, H, W = x.shape
         HW, rows = H * W, x.shape[0] * H * W
         C, D, Cc = self.mid_channels, self.depth_channels, self.context_channels

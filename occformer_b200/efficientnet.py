@@ -18,8 +18,8 @@ contract raises RuntimeError; there is no cuDNN fallback.  On CPU tensors ``forw
 ``_forward_torch`` (the oracle of the GPU tests), adaptive padding included.
 
 Stage outputs are handed on as the ResNet's are (image_encoder.py): an fp32 NCHW view of channel-last memory with the
-reference's channel count, carrying its S32 twin as ``_occ_s32``; the twin of a stage whose width is not a multiple of 32
-is zero-padded to whole chunks (SECONDFPN takes such twins).
+reference's channel count, carrying its S32 twin (common.attach_twin); the twin of a stage whose width is not a
+multiple of 32 is zero-padded to whole chunks (SECONDFPN takes such twins).
 """
 import math
 
@@ -28,7 +28,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import ops
-from .image_encoder import _batchnorm, _fold, _Prepared
+from .common import PreparedModule, attach_twin, batchnorm, fold_bn, round32
 from .registry import BACKBONES
 
 
@@ -77,7 +77,7 @@ class ConvBN(nn.Module):
     def __init__(self, cin, cout, k, stride=1, groups=1, norm_cfg=None, act=True):
         super().__init__()
         self.conv = Conv2dAdaptivePadding(cin, cout, k, stride, groups=groups, bias=False)
-        self.bn = _batchnorm(norm_cfg, cout, 1e-5)
+        self.bn = batchnorm(norm_cfg, cout, 1e-5)
         self.activate = Swish() if act else None
 
     def forward(self, x):
@@ -169,10 +169,6 @@ def scaled_layers(width, depth):
     return layers + [scaled[-1]]
 
 
-def _round32(c):
-    return (c + 31) // 32 * 32
-
-
 def _pad(t, *shape):
     """t zero-padded at the end of each dimension to shape"""
     out = t.new_zeros(shape)
@@ -181,7 +177,7 @@ def _pad(t, *shape):
 
 
 @BACKBONES.register_module()
-class CustomEfficientNet(_Prepared):
+class CustomEfficientNet(PreparedModule):
     """efficientnet.py:274-519 for the 'b' archs: forward(x (n, 3, H, W)) -> tuple of the layers in ``out_indices``
     (layer 0 = stem at stride 2, layers 1..5 the InvertedResidual stages at strides 2, 4, 8, 16, 32, layer 6 the 1x1 head
     conv).  The training-only kwargs (drop_path_rate, with_cp, frozen_stages, norm_eval) and init_cfg are accepted and
@@ -202,7 +198,7 @@ class CustomEfficientNet(_Prepared):
         if dict(act_cfg or {}).get("type") != "Swish":
             raise NotImplementedError(f"occformer_b200.CustomEfficientNet: act_cfg={act_cfg!r} is not supported "
                                       "(Swish only)")
-        _batchnorm(norm_cfg, 1, 1e-5)  # NotImplementedError naming norm_cfg for a non-BatchNorm norm
+        batchnorm(norm_cfg, 1, 1e-5)  # NotImplementedError naming norm_cfg for a non-BatchNorm norm
         if any(i not in range(7) for i in out_indices):
             raise ValueError(f"the item in out_indices must in range(0, 7). But received {tuple(out_indices)}")
         if frozen_stages not in range(8):
@@ -238,19 +234,18 @@ class CustomEfficientNet(_Prepared):
         "stem" (S32 (C0p, 32) in the im2col's (ky, kx, c) column order, bias), "blocks" one dict per InvertedResidual
         (expand / linear S32 (out, in) + bias, depthwise tap-major (k*k, C) + bias, SE K-major w1T (C, S), b1, w2T
         (S, C), b2), "head" (S32 (Cout, Cin), bias) of layers.6 when built.  Each block also records whether its output
-        is needed in S32 (the next op is a GEMM, or it ends a stage in out_indices).  Cached; a load_state_dict or .to()
-        drops the cache."""
+        is needed in S32 (the next op is a GEMM, or it ends a stage in out_indices)."""
         def fold(m):
-            return _fold(m.conv.weight, None, m.bn)
+            return fold_bn(m.conv.weight, None, m.bn)
 
         def gemm_w(w, b):  # 1x1 conv (Cout, Cin, 1, 1) -> S32 (Coutp, Cinp), bias (Coutp)
             co, ci = w.shape[:2]
-            return ops.split_weight(_pad(w[:, :, 0, 0], _round32(co), _round32(ci))), _pad(b, _round32(co))
+            return ops.split_weight(_pad(w[:, :, 0, 0], round32(co), round32(ci))), _pad(b, round32(co))
 
         w, b = fold(self.layers[0])
         c0, k = w.shape[0], w.shape[-1]
-        stem = ops.split_weight(_pad(w.permute(0, 2, 3, 1).reshape(c0, 3 * k * k), _round32(c0), 32))
-        P = {"stem": (stem, _pad(b, _round32(c0))), "blocks": [], "head": None}
+        stem = ops.split_weight(_pad(w.permute(0, 2, 3, 1).reshape(c0, 3 * k * k), round32(c0), 32))
+        P = {"stem": (stem, _pad(b, round32(c0))), "blocks": [], "head": None}
         stage_ends = {}
         for li, layer in enumerate(self.layers[1:], start=1):
             if not isinstance(layer, nn.Sequential):
@@ -258,7 +253,7 @@ class CustomEfficientNet(_Prepared):
                 continue
             for blk in layer:
                 mid, kk = blk.depthwise_conv.conv.weight.shape[0], blk.kernel_size
-                midp = _round32(mid)
+                midp = round32(mid)
                 wd, bd = fold(blk.depthwise_conv)
                 w1, w2 = blk.se.conv1.conv.weight[:, :, 0, 0].float(), blk.se.conv2.conv.weight[:, :, 0, 0].float()
                 sq = w1.shape[0]
@@ -275,7 +270,6 @@ class CustomEfficientNet(_Prepared):
             next_is_gemm = blocks[i + 1]["expand"] is not None if i + 1 < len(blocks) else P["head"] is not None
             p["stage"] = stage_ends.get(i)
             p["split"] = next_is_gemm or p["stage"] in self.out_indices
-        self._prep = P
         return P
 
     def _check_cuda_contract(self, x):
@@ -295,9 +289,7 @@ class CustomEfficientNet(_Prepared):
     def _stage(self, cur, cur_s, n, h, w, li):
         """fp32 rows (n*h*w, Cp) + S32 twin -> the NCHW view with the reference's channel count of layer li"""
         C = self._channels(li)
-        v = cur.view(n, h, w, -1)[..., :C].permute(0, 3, 1, 2)
-        v._occ_s32 = cur_s.view(n, h, w, -1)
-        return v
+        return attach_twin(cur.view(n, h, w, -1)[..., :C].permute(0, 3, 1, 2), cur_s.view(n, h, w, -1))
 
     def _channels(self, li):
         layer = self.layers[li]
@@ -307,7 +299,7 @@ class CustomEfficientNet(_Prepared):
     @torch.no_grad()
     def _forward_cuda(self, x):
         self._check_cuda_contract(x)
-        P = self._prep or self._prepare()
+        P = self.prepared()
         n, _, H, W = x.shape
         stem = self.layers[0].conv
         k, s = stem.weight.shape[-1], stem.stride[0]

@@ -11,12 +11,13 @@ all arithmetic runs in libocc_b200.so (wgmma GEMM / implicit-GEMM conv on split-
 passes per contraction, fp32-faithful --, fused norm / window attention / fusion kernels).  Inference (eval, no
 autograd) only.  Internally every tensor is channel-last (B,X,Y,Z,C); tensors that feed a tensor-core contraction are
 kept in the S32 split format (ops.py); returned tensors are fp32 permuted *views* with the reference's shape that carry
-their S32 twin as the attribute ``_occ_s32`` (the next module of this package picks it up instead of re-splitting).
+their S32 twin (common.attach_twin; the next module of this package picks it up instead of re-splitting).
 """
 import torch
 import torch.nn as nn
 
 from . import ops
+from .common import PreparedModule, attach_twin, twin_of
 from .registry import BACKBONES
 
 
@@ -99,7 +100,7 @@ class _BottleNeckASPP(nn.Module):
         self.output_conv = nn.Sequential(nn.Conv2d(ch, inplanes, 1, bias=False), nn.GroupNorm(ng, inplanes), nn.ReLU())
 
 
-class DualpathTransformerBlock(nn.Module):
+class DualpathTransformerBlock(PreparedModule):
     """dualpath_block.py:13-82.  ``layer_index`` decides the window shift (odd = shifted)."""
 
     def __init__(self, in_channels, channels, stride=1, norm_cfg=None, init_cfg=None, coeff_bias=True, aspp_drop=0.1,
@@ -121,15 +122,6 @@ class DualpathTransformerBlock(nn.Module):
         self.bev_encoder = _SwinBlock(channels, self.num_heads, self.shift)
         self.aspp = _BottleNeckASPP(channels, norm_cfg)
         self.combine_coeff = nn.Conv3d(channels, 1, 1, bias=coeff_bias)
-        self._prep = None
-        self.register_load_state_dict_post_hook(lambda m, k: m._invalidate())
-
-    def _invalidate(self):
-        self._prep = None
-
-    def _apply(self, fn, *a, **k):
-        self._prep = None
-        return super()._apply(fn, *a, **k)
 
     # ------------------------------------------------------------------ one-time weight preparation
     @torch.no_grad()
@@ -185,7 +177,6 @@ class DualpathTransformerBlock(nn.Module):
         P["w_a_out"], _ = ops.repack_conv_weight(a.output_conv[0].weight)
         P["coeff_w"] = self.combine_coeff.weight.detach().float().reshape(-1).contiguous()
         P["coeff_b"] = float(self.combine_coeff.bias.detach().float().item()) if self.combine_coeff.bias is not None else 0.0
-        self._prep = P
         return P
 
     # ------------------------------------------------------------------ forward on channel-last tensors
@@ -194,7 +185,7 @@ class DualpathTransformerBlock(nn.Module):
         """x_cl (B,X,Y,Z,Cin) contiguous channel-last fp32 (may be None when its S32 twin x_s is given)
         -> (out fp32 (B,X',Y',Z',C) | None, out S32): the S32 output feeds the next block / the neck, the fp32 one is
         only produced when the caller wants it (stage outputs)."""
-        P = self._prep or self._prepare()
+        P = self.prepared()
         if x_s is None:
             x_s = ops.to_split(x_cl)
         B, X0, Y0, Z0, Cin = x_s.shape
@@ -289,22 +280,16 @@ class DualpathTransformerBlock(nn.Module):
 def to_channel_last(x):
     """(B,C,X,Y,Z) reference-layout tensor (any strides) -> (contiguous (B,X,Y,Z,C) fp32, its S32 twin or None).
     Zero-copy when x is already a permuted view of channel-last memory (what this package's own modules hand around);
-    the S32 twin is the ``_occ_s32`` attribute such a view carries."""
+    the S32 twin is the one such a view carries (common.twin_of)."""
     if not x.is_cuda:
         raise RuntimeError("occformer_b200: the encoder runs on CUDA tensors only (no CPU fallback)")
-    twin = getattr(x, "_occ_s32", None)
-    x_cl = x.float().permute(0, 2, 3, 4, 1).contiguous()
-    if twin is not None and (twin.shape != x_cl.shape or twin.device != x_cl.device):
-        twin = None
-    return x_cl, twin
+    return x.float().permute(0, 2, 3, 4, 1).contiguous(), twin_of(x)
 
 
 def to_reference_layout(x_cl, x_s=None):
     """channel-last (B,X,Y,Z,C) -> the reference's (B,C,X,Y,Z) as a permuted view; the S32 twin rides along."""
     v = x_cl.permute(0, 4, 1, 2, 3)
-    if x_s is not None:
-        v._occ_s32 = x_s
-    return v
+    return v if x_s is None else attach_twin(v, x_s)
 
 
 @BACKBONES.register_module()

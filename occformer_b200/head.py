@@ -29,6 +29,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
+from .common import PreparedModule, twin_of
 from .dist_eval import PanopticEval
 from .registry import HEADS, POSITIONAL_ENCODING
 
@@ -107,7 +108,7 @@ class SinePositionalEncoding3D(nn.Module):
 
 
 # ------------------------------------------------------------------------------------------ the head
-class _Mask2FormerOccBase(nn.Module):
+class _Mask2FormerOccBase(PreparedModule):
     lidarseg = False
 
     def __init__(self, feat_channels, out_channels, num_occupancy_classes=20, num_queries=100,
@@ -161,15 +162,6 @@ class _Mask2FormerOccBase(nn.Module):
         self.sample_weight_gamma = sample_weight_gamma
         self.align_corners = True
         self.padding_mode = padding_mode
-        self._prep = None
-        self.register_load_state_dict_post_hook(lambda m, k: m._invalidate())
-
-    def _invalidate(self):
-        self._prep = None
-
-    def _apply(self, fn, *a, **k):
-        self._prep = None
-        return super()._apply(fn, *a, **k)
 
     # ------------------------------------------------------------------ one-time weight preparation
     @torch.no_grad()
@@ -209,7 +201,6 @@ class _Mask2FormerOccBase(nn.Module):
         P["vw"] = [ops.split_weight(cat(w)) if w else None for w in vw]
         P["kb"] = [cat(b) if b else None for b in kb]
         P["vb"] = [cat(b) if b else None for b in vb]
-        self._prep = P
         return P
 
     def _slots(self, w):
@@ -247,7 +238,7 @@ class _Mask2FormerOccBase(nn.Module):
     # ------------------------------------------------------------------ the decoder
     @torch.no_grad()
     def _decode(self, voxel_feats, keep_all_masks):
-        P = self._prep or self._prepare()
+        P = self.prepared()
         # Q = query slots of the kernels (rows per sample); Qr = real queries
         E, Q, Qr, H = self.decoder_embed_dims, self.num_slots, self.num_queries, self.num_heads
         nl, L, NC = self.num_transformer_feat_level, self.num_transformer_decoder_layers, self.num_classes + 1
@@ -259,8 +250,8 @@ class _Mask2FormerOccBase(nn.Module):
         scale = 32 ** -0.5
         # mask features: channel-last S32, produced once (operand of the 1+L mask GEMMs); the neck of this package hands
         # the S32 twin over directly
-        twin = getattr(mf, "_occ_s32", None)
-        if twin is not None and tuple(twin.shape) == (B, *grid, E) and twin.device == mf.device:
+        twin = twin_of(mf)
+        if twin is not None:
             mf_r = twin.view(B, V, E)
         else:
             x, cl = self._rows(mf)

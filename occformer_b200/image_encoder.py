@@ -16,7 +16,8 @@ their own (csrc/image_ops.cu).  A CUDA input outside that path's shape contract 
 fallback.  On CPU tensors ``forward`` is the plain torch restatement ``_forward_torch`` (the oracle of the GPU tests).
 
 Stage outputs are handed on as the package's other module boundaries are: an fp32 NCHW view of channel-last memory
-(torch's ``channels_last`` strides) carrying its S32 twin as ``_occ_s32``.  SECONDFPN picks the twin up; its own output is
+(torch's ``channels_last`` strides) carrying its S32 twin (common.attach_twin).  SECONDFPN picks the twin up while the
+level is unmodified (common.twin_of), else it splits the level itself; its own output is
 a ``channels_last`` map, which survives the reference glue's ``.view`` calls and which DepthNet splits without a
 transpose.
 
@@ -28,48 +29,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import ops
+from .common import PreparedModule, attach_twin, batchnorm, fold_bn, round32, twin_of
 from .registry import BACKBONES, NECKS
-
-_BN_TYPES = ("BN", "BN2d", "SyncBN", "NaiveSyncBN")  # identical in eval mode
-
-
-def _batchnorm(norm_cfg, channels, eps_default):
-    cfg = dict(norm_cfg or {})
-    kind = cfg.pop("type", "BN")
-    if kind not in _BN_TYPES:
-        raise NotImplementedError(f"occformer_b200: norm_cfg type {kind!r} is not supported (BatchNorm only)")
-    cfg.pop("requires_grad", None)
-    return nn.BatchNorm2d(channels, eps=cfg.get("eps", eps_default), momentum=cfg.get("momentum", 0.1))
-
-
-@torch.no_grad()
-def _fold(w, b, bn, out_dim=0):
-    """eval BatchNorm folded into the layer before it, in fp64, rounded to fp32: w' = w * g / sqrt(var + eps) along the
-    output dimension out_dim, b' = (b - mean) * g / sqrt(var + eps) + beta"""
-    s = bn.weight.double() / torch.sqrt(bn.running_var.double() + bn.eps)
-    b0 = b.double() if b is not None else torch.zeros_like(s)
-    shape = [1] * w.dim()
-    shape[out_dim] = -1
-    wf = (w.double() * s.view(shape)).float().contiguous()
-    return wf, ((b0 - bn.running_mean.double()) * s + bn.bias.double()).float().contiguous()
-
-
-class _Prepared(nn.Module):
-    """The cached-preparation pattern of the package's modules: ``_prepare()`` result kept until load_state_dict or
-    .to() / .cuda() / .double() drop it."""
-
-    def __init__(self):
-        super().__init__()
-        self._prep = None
-        self.register_load_state_dict_post_hook(lambda m, k: m._invalidate())
-
-    def _invalidate(self):
-        self._prep = None
-
-    def _apply(self, fn, *a, **k):
-        self._prep = None
-        return super()._apply(fn, *a, **k)
-
 
 # ---------------------------------------------------------------------------------------------------------- ResNet
 class Bottleneck(nn.Module):
@@ -80,11 +41,11 @@ class Bottleneck(nn.Module):
     def __init__(self, inplanes, planes, stride=1, downsample=None, norm_cfg=None):
         super().__init__()
         self.conv1 = nn.Conv2d(inplanes, planes, 1, bias=False)
-        self.bn1 = _batchnorm(norm_cfg, planes, 1e-5)
+        self.bn1 = batchnorm(norm_cfg, planes, 1e-5)
         self.conv2 = nn.Conv2d(planes, planes, 3, stride=stride, padding=1, bias=False)
-        self.bn2 = _batchnorm(norm_cfg, planes, 1e-5)
+        self.bn2 = batchnorm(norm_cfg, planes, 1e-5)
         self.conv3 = nn.Conv2d(planes, planes * self.expansion, 1, bias=False)
-        self.bn3 = _batchnorm(norm_cfg, planes * self.expansion, 1e-5)
+        self.bn3 = batchnorm(norm_cfg, planes * self.expansion, 1e-5)
         self.relu = nn.ReLU(inplace=True)
         self.downsample = downsample
         self.stride = stride
@@ -98,7 +59,7 @@ class Bottleneck(nn.Module):
 
 
 @BACKBONES.register_module(upstream=False)
-class ResNet(_Prepared):
+class ResNet(PreparedModule):
     """mmdet 2.14.0 ``ResNet`` at depth 50: forward(x (n, 3, H, W)) -> tuple of the stages in ``out_indices``, stage i
     with 64 * 2^(i+2) channels at stride 2^(i+2).
 
@@ -149,7 +110,7 @@ class ResNet(_Prepared):
         self.base_channels = base_channels
         self.stem_channels = stem_channels or base_channels
         self.conv1 = nn.Conv2d(3, self.stem_channels, 7, stride=2, padding=3, bias=False)
-        self.bn1 = _batchnorm(norm_cfg, self.stem_channels, 1e-5)
+        self.bn1 = batchnorm(norm_cfg, self.stem_channels, 1e-5)
         self.relu = nn.ReLU(inplace=True)
         self.maxpool = nn.MaxPool2d(kernel_size=3, stride=2, padding=1)
         self.res_layers = []
@@ -159,7 +120,7 @@ class ResNet(_Prepared):
             downsample = None
             if stride != 1 or inplanes != planes * Bottleneck.expansion:
                 downsample = nn.Sequential(nn.Conv2d(inplanes, planes * Bottleneck.expansion, 1, stride=stride, bias=False),
-                                           _batchnorm(norm_cfg, planes * Bottleneck.expansion, 1e-5))
+                                           batchnorm(norm_cfg, planes * Bottleneck.expansion, 1e-5))
             layer = [Bottleneck(inplanes, planes, stride, downsample, norm_cfg)]
             inplanes = planes * Bottleneck.expansion
             layer += [Bottleneck(inplanes, planes, 1, None, norm_cfg) for _ in range(1, blocks)]
@@ -177,28 +138,26 @@ class ResNet(_Prepared):
         """Eval BatchNorms folded into the convs before them (natural layouts, fp32 on the parameters' device):
         {"stem": (w (C0, 3, 7, 7), b), "blocks": [(stride, (w1, b1), (w2, b2), (w3, b3), (wd, bd) | None), ...]} with the
         blocks of all stages in order."""
-        F_ = {"stem": _fold(self.conv1.weight, None, self.bn1), "blocks": []}
+        F_ = {"stem": fold_bn(self.conv1.weight, None, self.bn1), "blocks": []}
         for name in self.res_layers:
             for blk in getattr(self, name):
                 ds = blk.downsample
-                F_["blocks"].append((blk.stride, _fold(blk.conv1.weight, None, blk.bn1), _fold(blk.conv2.weight, None, blk.bn2),
-                                     _fold(blk.conv3.weight, None, blk.bn3),
-                                     None if ds is None else _fold(ds[0].weight, None, ds[1])))
+                F_["blocks"].append((blk.stride, fold_bn(blk.conv1.weight, None, blk.bn1),
+                                     fold_bn(blk.conv2.weight, None, blk.bn2), fold_bn(blk.conv3.weight, None, blk.bn3),
+                                     None if ds is None else fold_bn(ds[0].weight, None, ds[1])))
         return F_
 
     @torch.no_grad()
     def _prepare(self):
         """The folded parameters in the kernels' layouts: the stem weight as a (C0, 160) S32 matrix in the im2col's
-        (ky, kx, c) column order (zero columns 147..159), the block convs repacked tap-major in S32.  Cached; a
-        load_state_dict or .to() drops the cache."""
+        (ky, kx, c) column order (zero columns 147..159), the block convs repacked tap-major in S32."""
         F_ = self._folded()
         w, b = F_["stem"]
         wm = w.permute(0, 2, 3, 1).reshape(w.shape[0], 147)
         wm = torch.cat([wm, wm.new_zeros(w.shape[0], ops.STEM_COLS - 147)], dim=1)
         rp = lambda wb: None if wb is None else (ops.repack_conv_weight(wb[0])[0], wb[1])  # noqa: E731
-        self._prep = {"stem": (ops.split_weight(wm), b),
-                      "blocks": [(s, rp(c1), rp(c2), rp(c3), rp(d)) for s, c1, c2, c3, d in F_["blocks"]]}
-        return self._prep
+        return {"stem": (ops.split_weight(wm), b),
+                "blocks": [(s, rp(c1), rp(c2), rp(c3), rp(d)) for s, c1, c2, c3, d in F_["blocks"]]}
 
     def _check_cuda_contract(self, x):
         need = []
@@ -219,7 +178,7 @@ class ResNet(_Prepared):
     @torch.no_grad()
     def _forward_cuda(self, x):
         self._check_cuda_contract(x)
-        P = self._prep or self._prepare()
+        P = self.prepared()
         n, _, H, W = x.shape
         stem = ops.gemm(ops.stem_im2col(x.float().contiguous()), P["stem"][0], bias=P["stem"][1], act=1)
         cur_s = ops.maxpool3x3s2(stem.view(n, H // 2, W // 2, -1)).unsqueeze(3)  # (n, H/4, W/4, 1, C0) S32
@@ -232,8 +191,7 @@ class ResNet(_Prepared):
             if si in self.out_indices:
                 nn_, h, w, _, C = cur.shape
                 v = cur.view(nn_, h, w, C).permute(0, 3, 1, 2)  # NCHW view, channels_last strides
-                v._occ_s32 = cur_s.view(nn_, h, w, C)
-                outs.append(v)
+                outs.append(attach_twin(v, cur_s.view(nn_, h, w, C)))
         return tuple(outs)
 
     @staticmethod
@@ -260,26 +218,13 @@ class ResNet(_Prepared):
 
 
 # ---------------------------------------------------------------------------------------------------------- SECONDFPN
-def _round32(c):
-    return (c + 31) // 32 * 32
-
-
-def _twin(t):
-    """the S32 twin (n, H, W, round_up(C, 32)) a backbone stage carries as ``_occ_s32`` (zero pad columns when C is not
-    a multiple of 32), or None"""
-    n, C, H, W = t.shape
-    t_s = getattr(t, "_occ_s32", None)
-    if t_s is None or t_s.shape != (n, H, W, _round32(C)) or t_s.device != t.device:
-        return None
-    return t_s
-
-
 @NECKS.register_module(upstream=False)
-class SECONDFPN(_Prepared):
+class SECONDFPN(PreparedModule):
     """second_fpn.py:11-91: one deblock per level -- ConvTranspose2d(kernel = stride = s) for an upsample stride s >= 1
     (s == 1 also Conv2d(1x1) with use_conv_for_no_stride), Conv2d(kernel = stride = 1/s) for s < 1 -- each followed by
     BatchNorm (default eps 1e-3) and ReLU; forward(levels) -> [channel concat of the deblock outputs].  On CUDA a level
-    whose width is not a multiple of 32 must carry its zero-padded S32 twin (CustomEfficientNet's stages do)."""
+    whose width is not a multiple of 32 must carry its zero-padded S32 twin and be unmodified since
+    (CustomEfficientNet's stages are handed over so)."""
 
     def __init__(self, in_channels=[128, 128, 256], out_channels=[256, 256, 256], upsample_strides=[1, 2, 4],
                  norm_cfg=dict(type="BN", eps=1e-3, momentum=0.01), upsample_cfg=dict(type="deconv", bias=False),
@@ -303,7 +248,7 @@ class SECONDFPN(_Prepared):
             else:
                 k = int(round(1 / stride))
                 layer = nn.Conv2d(in_channels[i], out_channel, kernel_size=k, stride=k, **cv)
-            deblocks.append(nn.Sequential(layer, _batchnorm(norm_cfg, out_channel, 1e-5), nn.ReLU(inplace=True)))
+            deblocks.append(nn.Sequential(layer, batchnorm(norm_cfg, out_channel, 1e-5), nn.ReLU(inplace=True)))
         self.deblocks = nn.ModuleList(deblocks)
 
     def forward(self, x):
@@ -322,7 +267,7 @@ class SECONDFPN(_Prepared):
         for blk in self.deblocks:
             layer, bn = blk[0], blk[1]
             deconv = isinstance(layer, nn.ConvTranspose2d)
-            w, b = _fold(layer.weight, layer.bias, bn, out_dim=1 if deconv else 0)
+            w, b = fold_bn(layer.weight, layer.bias, bn, out_dim=1 if deconv else 0)
             res.append(("deconv" if deconv else "conv", layer.stride[0], w, b))
         return res
 
@@ -330,10 +275,10 @@ class SECONDFPN(_Prepared):
     def _prepare(self):
         """The kernels' layouts: a conv (or a 1x1 deconv) as a tap-major S32 (Cout, f*f*Cin) matrix, the operand of a 1x1
         conv of the space_to_depth'd input; a stride-f deconv as the S32 (f*f*Cout, Cin) matrix whose row (i*f + j)*Cout
-        + o is w[:, o, i, j], with its bias repeated per (i, j).  Cached; a load_state_dict or .to() drops the cache."""
+        + o is w[:, o, i, j], with its bias repeated per (i, j)."""
         P = []
         for (kind, f, w, b), cin in zip(self._folded(), self.in_channels):
-            pad = _round32(cin) - cin  # zero input columns (per tap) for a level whose S32 twin is zero-padded
+            pad = round32(cin) - cin  # zero input columns (per tap) for a level whose S32 twin is zero-padded
             if kind == "conv":
                 P.append(("down", f, ops.repack_conv_weight(F.pad(w, (0, 0, 0, 0, 0, pad)))[0], b))
             elif f == 1:
@@ -341,7 +286,6 @@ class SECONDFPN(_Prepared):
             else:
                 P.append(("up", f, ops.split_weight(F.pad(w.permute(2, 3, 1, 0).reshape(-1, w.shape[0]), (0, pad))),
                           b.repeat(f * f)))
-        self._prep = P
         return P
 
     def _out_size(self, x):
@@ -356,9 +300,10 @@ class SECONDFPN(_Prepared):
         if any(t.dim() != 4 or t.shape[1] != c for t, c in zip(x, self.in_channels)):
             need.append(f"levels of shape (n, C_i, H_i, W_i) with C_i = {self.in_channels}")
         if any(c % 32 for c in self.out_channels) or (not need and any(
-                c % 32 and _twin(t) is None for t, c in zip(x, self.in_channels))):
+                c % 32 and twin_of(t) is None for t, c in zip(x, self.in_channels))):
             need.append("in_channels and out_channels multiples of 32 (whole 32-channel chunks; a narrower level must "
-                        "carry its S32 twin zero-padded to whole chunks, as CustomEfficientNet hands it over)")
+                        "carry its S32 twin zero-padded to whole chunks, as CustomEfficientNet hands it over, and be "
+                        "unmodified since)")
         if any(s not in (0.25, 0.5, 1, 2, 4) for s in self.upsample_strides):
             need.append("upsample_strides in {0.25, 0.5, 1, 2, 4}")
         if not need:
@@ -378,14 +323,14 @@ class SECONDFPN(_Prepared):
     @torch.no_grad()
     def _forward_cuda(self, x):
         self._check_cuda_contract(x)
-        P = self._prep or self._prepare()
+        P = self.prepared()
         n = x[0].shape[0]
         Ho, Wo = (int(v) for v in next(iter(self._out_size(x))))
         out = torch.empty((n * Ho * Wo, sum(self.out_channels)), dtype=torch.float32, device=x[0].device)
         off = 0
         for t, (kind, f, w, b), cout in zip(x, P, self.out_channels):
             _, C, H, W = t.shape
-            t_s = _twin(t)
+            t_s = twin_of(t)
             if t_s is None:
                 t_s = ops.split_nchw(t.float())
             C = t_s.shape[-1]

@@ -13,12 +13,13 @@ All arithmetic runs in libocc_b200.so: the 1x1x1 / 3x3x3 convolutions and the si
 wgmma GEMM (split-bf16 operands, three passes, fp32-faithful), the deformable gather / LayerNorm / FPN up-sampling in
 csrc/neck_ops.cu.  Tokens are kept level-major (csrc/neck_ops.cu) so that no concatenation, split or transpose of the
 reference's forward exists here; tensors that feed a contraction travel in the S32 split format and carry over from the
-encoder / to the head through the ``_occ_s32`` attribute.  Inference only.
+encoder / to the head as S32 twins (common.attach_twin).  Inference only.
 """
 import torch
 import torch.nn as nn
 
 from . import ops
+from .common import PreparedModule, attach_twin, twin_of
 from .head import SinePositionalEncoding3D, _get
 from .registry import ATTENTION, NECKS
 
@@ -71,7 +72,7 @@ class _Encoder(nn.Module):
 
 
 @NECKS.register_module()
-class MSDeformAttnPixelDecoder3D(nn.Module):
+class MSDeformAttnPixelDecoder3D(PreparedModule):
     def __init__(self, in_channels=[256, 512, 1024, 2048], strides=[4, 8, 16, 32], feat_channels=256, out_channels=256,
                  num_outs=3, conv_cfg=None, norm_cfg=None, act_cfg=None, encoder=None, positional_encoding=None,
                  init_cfg=None, **kwargs):
@@ -110,20 +111,11 @@ class MSDeformAttnPixelDecoder3D(nn.Module):
         self.output_convs = nn.ModuleList([_ConvGN(E, E, 3, False, G) for i in range(nin - L - 1, -1, -1)])
         self.mask_feature = nn.Conv3d(E, out_channels, 1)
         self.num_outs = num_outs
-        self._prep, self._pos = None, {}
-        self.register_load_state_dict_post_hook(lambda m, k: m._invalidate())
-
-    def _invalidate(self):
-        self._prep, self._pos = None, {}
-
-    def _apply(self, fn, *a, **k):
-        self._prep, self._pos = None, {}
-        return super()._apply(fn, *a, **k)
 
     @torch.no_grad()
     def _prepare(self):
         sw = ops.split_weight
-        P = {"in": [], "layers": [], "lat": [], "out": []}
+        P = {"in": [], "layers": [], "lat": [], "out": [], "pos": {}}
         for m in self.input_convs:
             P["in"].append(ops.repack_conv_weight(m.conv.weight)[0])
         for lyr in self.encoder.layers:
@@ -143,32 +135,31 @@ class MSDeformAttnPixelDecoder3D(nn.Module):
         for m in self.output_convs:
             P["out"].append(ops.repack_conv_weight(m.conv.weight))
         P["mf"] = ops.repack_conv_weight(self.mask_feature.weight)[0]
-        self._prep = P
         return P
 
-    def _pos_rows(self, grids, device):
-        """query_pos of the encoder (:160-163): sine encoding of every level + its level embedding, (Nq, E), cached per grid"""
+    def _pos_rows(self, P, grids, device):
+        """query_pos of the encoder (:160-163): sine encoding of every level + its level embedding, (Nq, E), cached per
+        grid in P["pos"]"""
         key = (tuple(grids), str(device))
-        if key not in self._pos:
+        if key not in P["pos"]:
             rows = [self.postional_encoding.rows(*g, device) + self.level_encoding.weight[i].detach().float()
                     for i, g in enumerate(grids)]
-            self._pos[key] = torch.cat(rows, 0).contiguous()
-        return self._pos[key]
+            P["pos"][key] = torch.cat(rows, 0).contiguous()
+        return P["pos"][key]
 
     @staticmethod
     def _operand(f):
         """(B,C,X,Y,Z) reference-layout tensor -> its channel-last S32 twin (picked up from the encoder, else split here)"""
         if not f.is_cuda:
             raise RuntimeError("occformer_b200: the neck runs on CUDA tensors only (no CPU fallback)")
-        B, C, X, Y, Z = f.shape
-        twin = getattr(f, "_occ_s32", None)
-        if twin is not None and tuple(twin.shape) == (B, X, Y, Z, C) and twin.device == f.device:
+        twin = twin_of(f)
+        if twin is not None:
             return twin
         return ops.to_split(f.float().permute(0, 2, 3, 4, 1).contiguous())
 
     @torch.no_grad()
     def forward(self, feats):
-        P = self._prep or self._prepare()
+        P = self.prepared()
         nin, L, E, G, H = self.num_input_levels, self.num_encoder_levels, self.embed_dims, self.groups, self.num_heads
         B = feats[0].shape[0]
         dev = feats[0].device
@@ -184,7 +175,7 @@ class MSDeformAttnPixelDecoder3D(nn.Module):
             st = ops.gn_stats(raw.view(B * ns[i], E), B, ns[i], E, G)
             ops.gn_apply(raw.view(B * ns[i], E), st, m.gn.weight, m.gn.bias, ns[i], G, relu=False,
                          out_f32=x[B * starts[i]:B * (starts[i] + ns[i])])
-        pos = self._pos_rows(grids, dev)
+        pos = self._pos_rows(P, grids, dev)
         strides = [self.strides[nin - i - 1] for i in range(L)]
         _, x_s, xq_s = ops.neck_token_prep(x, grids, B, pos=pos, want_f32=False, want_pos=True)
         # ---- DetrTransformerEncoder of BaseTransformerLayer('self_attn', 'norm', 'ffn', 'norm')  (:203-215)
@@ -225,7 +216,7 @@ class MSDeformAttnPixelDecoder3D(nn.Module):
         mf = ops.conv(mf_s, P["mf"], (1, 1, 1), bias=self.mask_feature.bias)
         outs[-1] = mf
         res = [o.permute(0, 4, 1, 2, 3) for o in outs[::-1]]
-        res[0]._occ_s32 = ops.to_split(mf)  # operand of the head's 1 + L mask GEMMs
+        attach_twin(res[0], ops.to_split(mf))  # operand of the head's 1 + L mask GEMMs
         return res
 
 

@@ -20,6 +20,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import ops
+from .common import PreparedModule, attach_twin
 from .depthnet import DepthNet
 from .registry import NECKS
 
@@ -43,7 +44,7 @@ def bev_pool(feats, coords, B, D, H, W):
 
 
 @NECKS.register_module()
-class ViewTransformerLiftSplatShootVoxel(nn.Module):
+class ViewTransformerLiftSplatShootVoxel(PreparedModule):
     def __init__(self, loss_depth_weight=1.0, grid_config=None, data_config=None, numC_input=512, numC_Trans=64,
                  downsample=16, point_cloud_range=None, loss_depth_type="bce", cam_channels=27, loss_depth_reg_weight=0.0,
                  use_voxel_net=False, accelerate=False, use_bev_pool=True, vp_megvii=False, vp_stero=False,
@@ -78,21 +79,15 @@ class ViewTransformerLiftSplatShootVoxel(nn.Module):
         self.point_cloud_range = point_cloud_range
         self.geom_feats = None
         self.accelerate, self.use_bev_pool, self.vp_megvii, self.vp_stereo = accelerate, use_bev_pool, vp_megvii, vp_stero
-        self._host = None
 
-    def _host_params(self):
-        # float copies of the tiny dx/bx/nx parameters for the by-value C ABI (one D2H, cached)
-        if self._host is None:
-            self._host = (self.dx.detach().cpu().tolist(), self.bx.detach().cpu().tolist(),
-                          self.nx.detach().cpu().tolist())
-        return self._host
+    def _prepare(self):
+        """(dx, bx, nx) as host float lists, the by-value arguments of the pooling kernels (one D2H)"""
+        return (self.dx.detach().cpu().tolist(), self.bx.detach().cpu().tolist(), self.nx.detach().cpu().tolist())
 
-    def _apply(self, fn, *a, **k):
-        self._host = None
-        return super()._apply(fn, *a, **k)
+    _host_params = PreparedModule.prepared  # the name bench.py reads them by
 
     def grid_size(self):
-        _, _, nx = self._host_params()
+        _, _, nx = self.prepared()
         return int(nx[0]), int(nx[1]), int(nx[2])
 
     def create_frustum(self):
@@ -166,7 +161,7 @@ class ViewTransformerLiftSplatShootVoxel(nn.Module):
     def voxel_pooling(self, geom_feats, x):
         """ViewTransformerLSSVoxel.py:77-100 with a materialised volume x (B,N,D,H,W,C).  -> (B,C,X,Y,Z) view."""
         B, N, D, H, W, C = x.shape
-        dx, bx, nx = self._host_params()
+        dx, bx, nx = self.prepared()
         feats = x.reshape(B * N * D * H * W, C).float().contiguous()
         geom = geom_feats.reshape(-1, 3).float().contiguous()
         out = ops.voxel_pool_geom(feats, geom, B, dx, bx, nx, self.grid_size())
@@ -176,7 +171,7 @@ class ViewTransformerLiftSplatShootVoxel(nn.Module):
     def lift_splat(self, depth_digit, img_feat, geom, B, N, with_split=False):
         """Fused lift-splat on post-DepthNet tensors: depth logits (B*N,D,fH,fW), context (B*N,C,fH,fW),
         geom (B,N,D,fH,fW,3).  Returns (channel-last grid (B,X,Y,Z,C) [or (grid, S32 twin) when with_split], depth_prob)."""
-        dx, bx, nx = self._host_params()
+        dx, bx, nx = self.prepared()
         prob, feat_cl = ops.lift_prologue(depth_digit.float().contiguous(), img_feat.float().contiguous())
         grid = ops.lift_splat(prob, feat_cl, geom.float().contiguous(), B, N, dx, bx, nx, self.grid_size(),
                               with_split=with_split)
@@ -197,11 +192,10 @@ class ViewTransformerLiftSplatShootVoxel(nn.Module):
         # depth softmax + get_geometry + voxel index + point lists + NHWC transpose in ONE front kernel, then the pooling
         # kernel (occ_lift_splat_fused); get_geometry / lift_splat stay available as separate calls
         split = self.numC_Trans % 32 == 0
-        dx, bx, nx = self._host_params()
+        dx, bx, nx = self.prepared()
         grid, depth_prob = ops.lift_splat_fused(depth_digit, img_feat, self.frustum.data, rots, trans, intrins, post_rots, post_trans, bda, B, N,
                                                 dx, bx, nx, self.grid_size(), with_split=split)
         if split:
-            out = grid[0].permute(0, 4, 1, 2, 3)
-            out._occ_s32 = grid[1]  # operand of the encoder's first conv (occformer_b200.encoder picks it up)
-            return out, depth_prob
+            # the S32 twin is the operand of the encoder's first conv (occformer_b200.encoder picks it up)
+            return attach_twin(grid[0].permute(0, 4, 1, 2, 3), grid[1]), depth_prob
         return grid.permute(0, 4, 1, 2, 3), depth_prob

@@ -176,7 +176,7 @@ def main():
         cams = {k: v.to(dev) for k, v in synth.nusc_cameras(1, 6).items()}
         dd, feat = synth.lift_inputs(1, 6, 112, 16, 44, C)
         dd, feat = dd.to(dev), feat.to(dev)
-        dx, bx, nx = vt._host_params()
+        dx, bx, nx = vt.prepared()
         t = timeit(lambda: ops.lift_splat_fused(dd, feat, vt.frustum.data, cams["rots"], cams["trans"], cams["intrins"],
                                                 cams["post_rots"], cams["post_trans"], cams["bda"], 1, 6, dx, bx, nx,
                                                 vt.grid_size(), with_split=True))

@@ -14,6 +14,7 @@ import torch.nn.functional as F
 from depthnet_ref import cam_gates, deform_cols, group_cols
 from util import GOLDEN, assert_close, parity_log, rel_err
 from occformer_b200 import ops, synth
+from occformer_b200.common import twin_of
 from occformer_b200.depthnet import DepthNet
 
 pytestmark = pytest.mark.gpu
@@ -234,7 +235,7 @@ def test_view_transformer_from_config(cuda, case):
     x = torch.randn(B, N, cin, fH, fW, generator=g)
     inp = [x.to(cuda)] + [cams[k].to(cuda) for k in ("rots", "trans", "intrins", "post_rots", "post_trans", "bda")]
     bev, prob = vt(inp + [mlp.to(cuda)])
-    assert getattr(bev, "_occ_s32", None) is not None and bev._occ_s32.shape == bev.permute(0, 2, 3, 4, 1).shape
+    assert twin_of(bev) is not None and twin_of(bev).shape == bev.permute(0, 2, 3, 4, 1).shape
     # CPU chain: torch DepthNet (fp64) -> oracle.port lift / voxel pooling
     out = _oracle(vt.depth_net, x.view(B * N, cin, fH, fW), mlp)
     vol, want_prob = port.lift(out[:, :D], out[:, D:D + ctx], B, N)

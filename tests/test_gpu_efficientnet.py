@@ -14,6 +14,7 @@ import torch.nn.functional as F
 
 from util import GOLDEN, assert_close, golden, parity_log, rel_err, rel_rms
 from occformer_b200 import BACKBONES, NECKS, ops, synth
+from occformer_b200.common import attach_twin, twin_of
 from occformer_b200.depthnet import DepthNet
 from occformer_b200.efficientnet import CustomEfficientNet, adaptive_pad
 from occformer_b200.image_encoder import SECONDFPN
@@ -189,7 +190,7 @@ def test_b7_full_size_against_fp64(cuda):
     for i, (o, wnt) in enumerate(zip(outs, want)):
         assert o.shape == wnt.shape
         C = o.shape[1]
-        assert o._occ_s32.shape[-1] == (C + 31) // 32 * 32
+        assert twin_of(o).shape[-1] == (C + 31) // 32 * 32
         r = assert_close(o, wnt, 1e-3, f"B7 stage {OUTS[i]}")
         pos = float((wnt > 0).double().mean())
         assert 0.05 < pos < 0.95, f"stage {OUTS[i]}: {pos:.1%} positive activations -- a vacuous comparison"
@@ -198,8 +199,9 @@ def test_b7_full_size_against_fp64(cuda):
     assert mid > 0.5, f"only {mid:.1%} of the SE gates are away from 0 / 1"
 
 
-def test_secondfpn_kitti_levels_against_fp64(cuda):
-    """the five KITTI levels with zero-padded S32 twins (48 -> 64, 80 -> 96) as CustomEfficientNet hands them over"""
+def test_secondfpn_kitti_levels_with_attached_twins_against_fp64(cuda):
+    """the five KITTI levels with zero-padded S32 twins (48 -> 64, 80 -> 96) handed over by attach_twin, as
+    CustomEfficientNet hands them over; a 48-wide level changed in place afterwards cannot be re-split and raises"""
     net = _neck(66, cuda)
     g = torch.Generator().manual_seed(67)
     n = 2
@@ -211,14 +213,16 @@ def test_secondfpn_kitti_levels_against_fp64(cuda):
         cp = (C + 31) // 32 * 32
         full = F.pad(t.permute(0, 2, 3, 1), (0, cp - C)).contiguous().to(cuda)
         v = full[..., :C].permute(0, 3, 1, 2)
-        v._occ_s32 = ops.to_split(full)
-        dev.append(v)
+        dev.append(attach_twin(v, ops.to_split(full)))
     y = net(dev)[0]
     assert y.shape == (n, 640, 24, 80)
     with torch.no_grad():
         want = _neck64(net)([t.double() for t in levels])[0]
     r = assert_close(y, want, 1e-3, "SECONDFPN KITTI levels")
     parity_log(f"[efficientnet] SECONDFPN at the KITTI levels: rel_max {r:.2e}")
+    dev[0].mul_(0.5)
+    with pytest.raises(RuntimeError, match="unmodified since"):
+        net(dev)
 
 
 def test_images_to_view_transformer(cuda):

@@ -14,6 +14,7 @@ import torch.nn.functional as F
 
 from util import GOLDEN, assert_close, parity_log, rel_err, rel_rms
 from occformer_b200 import BACKBONES, NECKS, ops, synth
+from occformer_b200.common import attach_twin, twin_of
 from occformer_b200.depthnet import DepthNet
 from occformer_b200.image_encoder import SECONDFPN, ResNet
 
@@ -155,16 +156,17 @@ def test_resnet50_against_fp64(cuda):
     assert len(outs) == 4
     for i, (o, w) in enumerate(zip(outs, want)):
         assert o.shape == w.shape and o.is_contiguous(memory_format=torch.channels_last)
-        assert torch.equal(_bits(o._occ_s32), _bits(ops.to_split(o.permute(0, 2, 3, 1).contiguous())))
+        assert torch.equal(_bits(twin_of(o)), _bits(ops.to_split(o.permute(0, 2, 3, 1).contiguous())))
         r = assert_close(o, w, 1e-3, f"ResNet-50 stage {i}")
         pos = float((w > 0).double().mean())
         assert 0.05 < pos < 0.95, f"stage {i}: {pos:.1%} positive activations -- a vacuous comparison"
         parity_log(f"[image encoder] ResNet-50 (6, 3, 256, 704) stage {i}: rel_max {r:.2e}, {pos:.0%} positive")
 
 
-@pytest.mark.parametrize("twin", [True, False])
+@pytest.mark.parametrize("twin", [True, False, "modified"])
 def test_secondfpn_against_fp64(cuda, twin):
-    """at R50 shapes: levels with their S32 twin (as the ResNet hands them over), and plain NCHW levels"""
+    """at R50 shapes: levels with their S32 twin (as the ResNet hands them over), plain NCHW levels, and levels with
+    twins of which one was scaled in place after the hand-over (its twin is stale: SECONDFPN must split the level)"""
     net = _neck(10, cuda)
     g = torch.Generator().manual_seed(11)
     n = 6
@@ -174,8 +176,11 @@ def test_secondfpn_against_fp64(cuda, twin):
         d = t.to(cuda)
         if twin:
             d = d.permute(0, 2, 3, 1).contiguous().permute(0, 3, 1, 2)
-            d._occ_s32 = ops.to_split(d.permute(0, 2, 3, 1).contiguous())
+            attach_twin(d, ops.to_split(d.permute(0, 2, 3, 1).contiguous()))
         dev_levels.append(d)
+    if twin == "modified":
+        dev_levels[1].mul_(0.5)
+        levels[1] = levels[1] * 0.5
     out = net(dev_levels)
     assert isinstance(out, list) and len(out) == 1
     y = out[0]
@@ -183,7 +188,7 @@ def test_secondfpn_against_fp64(cuda, twin):
     with torch.no_grad():
         want = _neck64(net)([t.double() for t in levels])[0]
     r = assert_close(y, want, 1e-3, f"SECONDFPN R50 twin={twin}")
-    parity_log(f"[image encoder] SECONDFPN R50 (twin={int(twin)}): rel_max {r:.2e}")
+    parity_log(f"[image encoder] SECONDFPN R50 (twin={twin if isinstance(twin, str) else int(twin)}): rel_max {r:.2e}")
 
 
 def test_secondfpn_other_strides(cuda):

@@ -107,8 +107,9 @@ def test_neck_vs_reference_golden_and_port(cuda, B):
             assert_close(o, torch.from_numpy(gold[f"out{i}"]), what=f"neck out[{i}] vs reference golden")
     # the S32 twin handed to the head equals split(mask_feature)
     from occformer_b200 import ops
+    from occformer_b200.common import twin_of
     mf = outs[0].permute(0, 2, 3, 4, 1).contiguous()
-    assert torch.equal(ops.to_split(mf).view(torch.int32), outs[0]._occ_s32.view(torch.int32))
+    assert torch.equal(ops.to_split(mf).view(torch.int32), twin_of(outs[0]).view(torch.int32))
 
 
 def test_neck_full_width_pr1_grid(cuda):

@@ -7,6 +7,7 @@ import torch
 
 from oracle import port
 from occformer_b200 import synth
+from occformer_b200.common import twin_of
 from util import assert_close, golden
 
 pytestmark = pytest.mark.gpu
@@ -257,5 +258,5 @@ def test_forward_fused_front_end_vs_oracle(cuda, wl, B):
     if int(flips.sum()) == 0:
         assert_close(voxel, ref, 1e-4, f"{wl} forward pooled grid")  # fp32 exp + summation-order noise on near-cancelling sums
         assert torch.equal(ops.to_split(voxel.permute(0, 2, 3, 4, 1).contiguous()).view(torch.int32),
-                           voxel._occ_s32.view(torch.int32))
+                           twin_of(voxel).view(torch.int32))
     print(f"{wl}: forward front-end flips {int(flips.sum())} of {flips.numel()}")
