@@ -17,7 +17,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
@@ -26,6 +25,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from occformer_b200 import synth  # noqa: E402
 from occformer_b200.depthnet import DepthNet  # noqa: E402
 from occformer_b200.view_transformer import ViewTransformerLiftSplatShootVoxel  # noqa: E402
+from gpu_bench import alternated, capture, card, rel, torch_arms  # noqa: E402
 
 CIN, MID, CTX, D, CAM, N, FH, FW = 512, 512, 128, 112, 27, 6, 16, 44
 
@@ -41,32 +41,6 @@ def depthnet_flops(n, H, W, cin=CIN, mid=MID, ctx=CTX, d=D):
             + 9 * mid * mid // 4       # DCN, 4 groups
             + mid * d)                 # depth head 1x1
     return 2.0 * macs * n * H * W
-
-
-def card():
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unknown card"
-
-
-def graphed(fn):
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            fn()
-    torch.cuda.current_stream().wait_stream(s)
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        out = fn()
-    torch.cuda.synchronize()
-    return g, out
-
-
-def rel(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).abs().max() / b.abs().max().clamp_min(1e-30))
 
 
 def main():
@@ -88,16 +62,6 @@ def main():
     mlp_h = torch.randn(B, N, CAM, generator=g)
     x, mlp = x_h.to(dev), mlp_h.to(dev)
 
-    tf32 = (torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32)
-
-    def torch_arm(allow):
-        def run():
-            torch.backends.cudnn.allow_tf32 = allow
-            torch.backends.cuda.matmul.allow_tf32 = allow and tf32[1]
-            with torch.no_grad():
-                return net._forward_torch(x, mlp)
-        return run
-
     # view transformer (library DepthNet + fused lift-splat) at the reference grid 128 x 128 x 16
     vt = ViewTransformerLiftSplatShootVoxel(grid_config=synth.grid_config("nusc_ref"), data_config={"input_size": (256, 704)},
                                             numC_input=CIN, numC_Trans=CTX, cam_channels=CAM)
@@ -107,25 +71,9 @@ def main():
     vt_in = [x.view(B, N, CIN, FH, FW)] + [cams[k] for k in ("rots", "trans", "intrins", "post_rots", "post_trans", "bda")]
     vt_in.append(mlp)
 
-    arms = {"library": lambda: net(x, mlp), "torch_tf32": torch_arm(True), "torch_fp32": torch_arm(False),
-            "view_transformer": lambda: vt(vt_in)[0]}
-    graphs, outs = {}, {}
-    for name, fn in arms.items():
-        graphs[name], outs[name] = graphed(fn)
-    torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = tf32
-
-    flush = torch.empty(128 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)
-    times = {k: [] for k in graphs}
-    for it in range(args.warmup + args.iters):
-        for name, gr in graphs.items():
-            flush.zero_()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            gr.replay()
-            e1.record()
-            e1.synchronize()
-            if it >= args.warmup:
-                times[name].append(e0.elapsed_time(e1))
+    graphs, outs = capture({"library": lambda: net(x, mlp), **torch_arms(lambda: net._forward_torch(x, mlp)),
+                            "view_transformer": lambda: vt(vt_in)[0]})
+    times = alternated(graphs, args.iters, args.warmup)
 
     ref = DepthNet(CIN, MID, CTX, D, cam_channels=CAM).eval()
     ref.load_state_dict(sd, strict=True)

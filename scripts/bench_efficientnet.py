@@ -18,21 +18,20 @@ profiled eager forward), and the card name, power limit and max SM clock read in
 GPU.
 """
 import argparse
-import collections
 import copy
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
 import torch.nn as nn
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from occformer_b200 import ops, synth  # noqa: E402
+from occformer_b200 import synth  # noqa: E402
 from occformer_b200.efficientnet import CustomEfficientNet  # noqa: E402
 from occformer_b200.image_encoder import SECONDFPN  # noqa: E402
+from gpu_bench import alternated, capture, card, launch_shares, rel, torch_arms  # noqa: E402
 
 H, W = 384, 1280
 OUTS = (2, 3, 4, 5, 6)
@@ -59,55 +58,8 @@ def encoder_flops(net, neck, n, h=H, w=W):
     return 2.0 * macs * n
 
 
-def card():
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unknown card"
-
-
-def graphed(fn):
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(2):
-            fn()
-    torch.cuda.current_stream().wait_stream(s)
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        out = fn()
-    torch.cuda.synchronize()
-    return g, out
-
-
-def rel(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).abs().max() / b.abs().max().clamp_min(1e-30))
-
-
 KINDS = (("stem_im2col", "stem_im2col"), ("depthwise", "dwconv_swish"), ("se_gate", "se_gate"), ("se_scale", "se_scale"),
          ("to_split", "split_rows"), ("fpn_glue", "space_to_depth|depth_to_space|head_prep"), ("gemm", "gemm_bf16x3"))
-
-
-def launch_shares(fn):
-    """GPU time per kind of launch of one eager call of fn (torch.profiler), in ms"""
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        n0 = ops.LAUNCH_COUNT[0]
-        fn()
-        torch.cuda.synchronize()
-        launches = ops.LAUNCH_COUNT[0] - n0
-    t = collections.defaultdict(float)
-    cnt = collections.Counter()
-    for e in prof.events():
-        if not str(e.device_type).endswith("CUDA"):
-            continue
-        kind = next((k for k, pat in KINDS if any(p in e.name for p in pat.split("|"))), "other")
-        t[kind] += e.device_time_total / 1e3 if hasattr(e, "device_time_total") else e.cuda_time_total / 1e3
-        cnt[kind] += 1
-    total = sum(t.values())
-    return launches, {k: {"launches": cnt[k], "ms": round(t[k], 3), "share": round(t[k] / total, 4)} for k in t}
 
 
 def main():
@@ -130,39 +82,14 @@ def main():
     x_h = torch.randn(n, 3, H, W, generator=torch.Generator().manual_seed(2))
     x = x_h.to(dev)
 
-    tf32 = (torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32)
-
-    def torch_arm(allow):
-        def run():
-            torch.backends.cudnn.allow_tf32 = allow
-            torch.backends.cuda.matmul.allow_tf32 = allow and tf32[1]
-            with torch.no_grad():
-                return neck._forward_torch(list(backbone._forward_torch(x)))[0]
-        return run
-
     def library():
         return neck(list(backbone(x)))[0]
 
-    arms = {"library": library, "torch_tf32": torch_arm(True), "torch_fp32": torch_arm(False)}
-    graphs, outs = {}, {}
-    for name, fn in arms.items():
-        graphs[name], outs[name] = graphed(fn)
-    torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = tf32
+    graphs, outs = capture({"library": library,
+                            **torch_arms(lambda: neck._forward_torch(list(backbone._forward_torch(x)))[0])})
+    times = alternated(graphs, args.iters, args.warmup)
 
-    flush = torch.empty(128 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)
-    times = {k: [] for k in graphs}
-    for it in range(args.warmup + args.iters):
-        for name, gr in graphs.items():
-            flush.zero_()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            gr.replay()
-            e1.record()
-            e1.synchronize()
-            if it >= args.warmup:
-                times[name].append(e0.elapsed_time(e1))
-
-    launches, shares = launch_shares(library)
+    launches, shares = launch_shares(library, KINDS)
     rb, rn = copy.deepcopy(backbone).double(), copy.deepcopy(neck).double()
     with torch.no_grad():
         want = rn._forward_torch(list(rb._forward_torch(x[:1].double())))[0]

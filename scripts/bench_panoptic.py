@@ -7,11 +7,10 @@
    head (150 queries) and the semantic head (100 queries) alternate in one run.
 2. The panoptic tail alone (occ_panoptic_voxels on the last layer's native logits), with its algorithmic bytes over the
    time against the H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s), next to the semantic tail (occ_classmix).
-Prints the card name and power limit with the numbers.  Needs a GPU; there is no CPU fallback.
+Prints the card name, power limit and max SM clock with the numbers.  Needs a GPU; there is no CPU fallback.
 """
 import argparse
 import os
-import subprocess
 import sys
 
 import torch
@@ -20,14 +19,9 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench  # noqa: E402
 from occformer_b200 import HEADS, ops, synth  # noqa: E402
 from occformer_b200.head import head_cfg  # noqa: E402
+from gpu_bench import card  # noqa: E402
 
 HBM_TBS = 3.35
-
-
-def card():
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unknown card"
 
 
 def build_head(dev, wl, queries):

@@ -5,12 +5,11 @@ restatement of the reference's per-class np.unique algorithm (oracle/panoptic_ev
 
 Inputs: one 256x256x32 voxel scan (~5000 thing instances, 20 % ignored) and one 34 720-point LiDAR scan, int64 on the
 device.  Device time per addBatch with CUDA events, L2 flushed before every call; host time of the restatement on the
-same inputs already in host memory (the device-to-host copy is not counted).  Prints the card name and power limit and
-the host's core count with the numbers.  Needs a GPU; there is no CPU fallback.
+same inputs already in host memory (the device-to-host copy is not counted).  Prints the card name, power limit and max
+SM clock and the host's core count with the numbers.  Needs a GPU; there is no CPU fallback.
 """
 import argparse
 import os
-import subprocess
 import sys
 import time
 
@@ -20,12 +19,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from occformer_b200.dist_eval import PanopticEval  # noqa: E402
 from oracle import panoptic_eval as pe  # noqa: E402
-
-
-def card():
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unknown card"
+from gpu_bench import card  # noqa: E402
 
 
 def device_ms(scan, iters, flush):

@@ -2,17 +2,13 @@
 the camera-aware SE gates, their application, the deformable im2col, the whole module and the view transformer that
 runs it.  The oracle is depthnet.py's torch forward on the host in float64 (pinned to the reference class by
 test_depthnet_vs_reference_golden) and the plain restatements of tests/depthnet_ref.py."""
-import json
-import os
-import subprocess
-import sys
-
 import pytest
 import torch
 import torch.nn.functional as F
 
 from depthnet_ref import cam_gates, deform_cols, group_cols
-from util import GOLDEN, assert_close, parity_log, rel_err
+from util import assert_close, f64, parity_log, rel_err, run_trace
+from vt_chain import check_pooled, config_view_transformer
 from occformer_b200 import ops, synth
 from occformer_b200.common import twin_of
 from occformer_b200.depthnet import DepthNet
@@ -30,14 +26,6 @@ def _net(cin, mid, ctx, D, cam, seed, dev):
     net = DepthNet(cin, mid, ctx, D, cam_channels=cam).eval()
     net.load_state_dict(synth.make_depthnet_state(cin, mid, ctx, D, cam, seed=seed), strict=True)
     return net.to(dev)
-
-
-def _oracle(net, x, mlp):
-    """depthnet.py's torch forward in float64 on the host"""
-    ref = DepthNet(net.in_channels, net.mid_channels, net.context_channels, net.depth_channels, net.cam_channels).eval()
-    ref.load_state_dict({k: v.cpu() for k, v in net.state_dict().items()})
-    with torch.no_grad():
-        return ref.double()(x.cpu().double(), mlp.cpu().double())
 
 
 # ------------------------------------------------------------------ 1. conv into a column slice
@@ -121,9 +109,7 @@ def test_cam_gates_against_fp64(cuda, cam, C):
     r = assert_close(gates, want, KERNEL_TOL, f"cam gates cam={cam} C={C}")
     parity_log(f"[depthnet] cam gates cam={cam}: rel_max {r:.2e}")
     # against the module's own Mlp / SELayer chain (BatchNorm1d not folded), fp64
-    ref = DepthNet(64, C, 32, 16, cam_channels=cam).eval()
-    ref.load_state_dict({k: v.cpu() for k, v in net.state_dict().items()})
-    ref = ref.double()
+    ref = f64(net)
     with torch.no_grad():
         mm = ref.bn(m.double())
         for i, (mlp, se) in enumerate(((ref.depth_mlp, ref.depth_se), (ref.context_mlp, ref.context_se))):
@@ -207,7 +193,8 @@ def test_depthnet_against_fp64(cuda, case):
     net = _net(cin, mid, ctx, D, cam, 13, cuda)
     x, mlp = _inputs(case)
     y = net(x.to(cuda), mlp.to(cuda))
-    want = _oracle(net, x, mlp)
+    with torch.no_grad():
+        want = f64(net)(x.double(), mlp.double())
     rd = assert_close(y[:, :D], want[:, :D], 1e-3, f"DepthNet {case} depth logits")
     rc = assert_close(y[:, D:], want[:, D:], 1e-3, f"DepthNet {case} context")
     parity_log(f"[depthnet] {case}: depth rel_max {rd:.2e}, context rel_max {rc:.2e}")
@@ -216,64 +203,23 @@ def test_depthnet_against_fp64(cuda, case):
 # ------------------------------------------------------------------ 6. connected: the view transformer from the config
 @pytest.mark.parametrize("case", ["nusc_r50", "kitti"])
 def test_view_transformer_from_config(cuda, case):
-    from oracle import port
-    from occformer_b200 import NECKS
-    cfg = json.load(open(os.path.join(GOLDEN, f"model_cfg_{case}.json")))["img_view_transformer"]
-    vt = NECKS.build(cfg)
     cin, mid, ctx, D, cam, B, N, fH, fW = CASES[case]
-    assert (vt.numC_input, vt.cam_channels, vt.D, vt.numC_Trans) == (cin, cam, D, ctx)
-    sd = synth.make_depthnet_state(cin, mid, ctx, D, cam, seed=14)
-    cams = synth.workload_cameras("kitti" if case == "kitti" else "nusc_ref", B)
-    mlp = vt.get_mlp_input(cams["rots"], cams["trans"], cams["intrins"], cams["post_rots"], cams["post_trans"],
-                           cams["bda"])
-    # running statistics of mlp_input's BatchNorm1d that match these cameras (as a trained model's would)
-    sd["bn.running_mean"] = mlp.reshape(-1, cam).mean(0)
-    sd["bn.running_var"] = mlp.reshape(-1, cam).var(0, unbiased=False) + 1.0
-    vt.depth_net.load_state_dict(sd, strict=True)
-    vt = vt.to(cuda).eval()
+    vt, cams, mlp = config_view_transformer(case, 14, B)
+    assert (vt.numC_input, vt.depth_net.mid_channels, vt.cam_channels, vt.D, vt.numC_Trans) == (cin, mid, cam, D, ctx)
+    vt = vt.to(cuda)
     g = torch.Generator().manual_seed(15)
     x = torch.randn(B, N, cin, fH, fW, generator=g)
     inp = [x.to(cuda)] + [cams[k].to(cuda) for k in ("rots", "trans", "intrins", "post_rots", "post_trans", "bda")]
     bev, prob = vt(inp + [mlp.to(cuda)])
     assert twin_of(bev) is not None and twin_of(bev).shape == bev.permute(0, 2, 3, 4, 1).shape
-    # CPU chain: torch DepthNet (fp64) -> oracle.port lift / voxel pooling
-    out = _oracle(vt.depth_net, x.view(B * N, cin, fH, fW), mlp)
-    vol, want_prob = port.lift(out[:, :D], out[:, D:D + ctx], B, N)
-    gc = vt.grid_config
-    frustum = port.create_frustum(vt.data_config["input_size"], vt.downsample, gc["dbound"])
-    geom = port.get_geometry(frustum, **cams)
-    dx, bx, nx = port.gen_dx_bx(gc["xbound"], gc["ybound"], gc["zbound"])
-    _, gf, kept = port.voxel_pooling(geom, vol[..., :1], dx, bx, nx)
-    # the kernel recomputes the geometry in fp32: a point may change voxel only within 1e-4 cells of a cell boundary;
-    # the oracle sums are taken over the kernel's voxel assignment so that such a point does not decide the comparison
-    X, Y, Z = vt.grid_size()
-    vox = ops._workspace(gf.shape[0], B, X, Y, Z, cuda).vox_id.cpu().long()
-    ref_lin = ((gf[:, 3] * X + gf[:, 0]) * Y + gf[:, 1]) * Z + gf[:, 2]
-    flips = vox != torch.where(kept, ref_lin, torch.full_like(ref_lin, -1))
-    frac = (geom.view(-1, 3) - (bx - dx / 2.0)) / dx
-    assert bool((~flips | ((frac - frac.round()).abs() < 1e-4).any(-1)).all()), "index flips away from cell boundaries"
-    rows = vol.reshape(-1, ctx)
-    keep = vox >= 0
-    want = torch.zeros(B * X * Y * Z, ctx, dtype=torch.float64).index_add_(0, vox[keep], rows[keep])
-    want = want.view(B, X, Y, Z, ctx).permute(0, 4, 1, 2, 3)
-    rp = assert_close(prob, want_prob, 1e-3, f"view transformer {case} depth_prob")
-    rg = assert_close(bev, want, 1e-3, f"view transformer {case} pooled grid")
-    parity_log(f"[depthnet] view transformer {case}: depth_prob rel_max {rp:.2e}, grid rel_max {rg:.2e}, "
-               f"{int(flips.sum())} boundary flips of {flips.numel()} points")
+    with torch.no_grad():
+        out = f64(vt.depth_net)(x.view(B * N, cin, fH, fW).double(), mlp.double())
+    check_pooled(vt, cams, out, prob, bev, B, N, f"[depthnet] view transformer {case}", "exact")
 
 
 # ------------------------------------------------------------------ 7. only library kernels, graph-safe
 def test_only_library_kernels_and_cuda_graph(cuda):
-    """tests/depthnet_trace.py in a process of its own: its profiler session and graph capture must not change what a
-    later profiler session of this process records (test_gpu_launch_count compares a trace with the launch counter)"""
-    here = os.path.dirname(os.path.abspath(__file__))
-    flags = ["-s"] if sys.flags.no_user_site else []  # the same interpreter settings as this process
-    r = subprocess.run([sys.executable, *flags, os.path.join(here, "depthnet_trace.py")], capture_output=True, text=True,
-                       timeout=600)
-    assert r.returncode == 0, f"depthnet_trace.py failed:\n{r.stdout}\n{r.stderr}"
-    res = json.loads(r.stdout.strip().splitlines()[-1])
-    print(f"[depthnet launches] counted {res['counted']}, trace: {res['kernels']} occ:: kernels + {res['memsets']} memsets")
-    assert not res["other"], f"non-library GPU work: {res['other'][:5]}"
+    res = run_trace("depthnet", 600)
     assert res["counted"] == res["kernels"] + res["memsets"] and 20 <= res["counted"] <= 40
     assert res["graph_equals_eager"], "CUDA-graph replay differs from the eager forward"
 
@@ -285,7 +231,8 @@ def test_bf16_mode(cuda):
     x, mlp = _inputs("nusc_r50", seed=19)
     with ops.precision("bf16"):
         y = net(x.to(cuda), mlp.to(cuda))
-    want = _oracle(net, x, mlp)
+    with torch.no_grad():
+        want = f64(net)(x.double(), mlp.double())
     rd = assert_close(y[:, :D], want[:, :D], 3e-2, "DepthNet bf16 depth logits")
     rc = assert_close(y[:, D:], want[:, D:], 3e-2, "DepthNet bf16 context")
     parity_log(f"[depthnet] bf16 mode: depth rel_max {rd:.2e}, context rel_max {rc:.2e}")

@@ -2,20 +2,17 @@
 the Swish epilogue and the generalised stem im2col one launch at a time, single blocks, the whole B7 at the SemanticKITTI
 size, SECONDFPN at the KITTI levels, and the chain images -> B7 -> SECONDFPN -> view transformer.  The oracle is
 efficientnet.py's torch forward in float64 (pinned to the reference class by tests/test_cpu_efficientnet.py)."""
-import copy
 import json
 import os
-import subprocess
-import sys
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from util import GOLDEN, assert_close, golden, parity_log, rel_err, rel_rms
+from util import GOLDEN, assert_close, bits, f64, golden, images, parity_log, rel_err, rel_rms, run_trace
+from vt_chain import check_pooled, config_view_transformer
 from occformer_b200 import BACKBONES, NECKS, ops, synth
 from occformer_b200.common import attach_twin, twin_of
-from occformer_b200.depthnet import DepthNet
 from occformer_b200.efficientnet import CustomEfficientNet, adaptive_pad
 from occformer_b200.image_encoder import SECONDFPN
 
@@ -24,10 +21,7 @@ pytestmark = pytest.mark.gpu
 KERNEL_TOL = 5e-5
 OUTS = (2, 3, 4, 5, 6)
 FPN = dict(in_channels=[48, 80, 224, 640, 2560], out_channels=[128] * 5, upsample_strides=[0.25, 0.5, 1, 2, 2])
-
-
-def _bits(t):
-    return t.detach().contiguous().view(torch.int32).cpu()
+HW = (384, 1280)
 
 
 def _b7(seed, dev, out_indices=OUTS):
@@ -36,27 +30,10 @@ def _b7(seed, dev, out_indices=OUTS):
     return net.to(dev)
 
 
-def _f64(net, dev=None):
-    """the same module in float64 (the oracle), on the host or -- for full-size B7 -- on `dev`, run through its torch
-    forward (fp64 convolutions, no TF32)"""
-    ref = copy.deepcopy(net).cpu().double().eval()
-    return ref.to(dev) if dev is not None else ref
-
-
 def _neck(seed, dev):
     net = SECONDFPN(**FPN).eval()
     net.load_state_dict(synth.make_secondfpn_state(seed=seed, out_hw=(6, 20), **FPN), strict=True)
     return net.to(dev)
-
-
-def _neck64(net):
-    ref = SECONDFPN(net.in_channels, net.out_channels, net.upsample_strides).eval()
-    ref.load_state_dict({k: v.cpu() for k, v in net.state_dict().items()})
-    return ref.double()
-
-
-def _images(n, H=384, W=1280, seed=0):
-    return torch.randn(n, 3, H, W, generator=torch.Generator().manual_seed(seed))
 
 
 def _swish(x):
@@ -87,7 +64,7 @@ def test_dwconv_swish_against_fp64(cuda, k, s, C, H, W):
     parity_log(f"[efficientnet] depthwise k{k} s{s} C{C} {H}x{W}: rel_max {r:.2e}, SE sums {rs:.2e}")
     # fixed-order partials: a second launch is bit-identical
     y2, part2 = ops.dwconv_swish(x_cl, wt, b.to(cuda), k, s, pt, pl, Ho, Wo)
-    assert torch.equal(_bits(y2), _bits(y)) and torch.equal(_bits(part2), _bits(part))
+    assert torch.equal(bits(y2), bits(y)) and torch.equal(bits(part2), bits(part))
 
 
 @pytest.mark.parametrize("C,S,hw", [(288, 12, 1920), (1344, 56, 480), (64, 16, 122880), (3840, 160, 480)])
@@ -124,8 +101,8 @@ def test_swish_epilogue_against_fp64(cuda):
     r = assert_close(y, want, KERNEL_TOL, "GEMM Swish epilogue")
     x_s = ops.to_split(a.view(10, 10, 10, 1, K).to(cuda))
     yc = ops.conv(x_s, ops.repack_conv_weight(w.view(N, K, 1, 1).to(cuda))[0], (1, 1, 1), bias=b.to(cuda), act=3)
-    assert torch.equal(_bits(yc.view(M, N)), _bits(ops.gemm(ops.to_split(a.to(cuda)), ops.split_weight(w).to(cuda),
-                                                           bias=b.to(cuda), act=3)))
+    assert torch.equal(bits(yc.view(M, N)), bits(ops.gemm(ops.to_split(a.to(cuda)), ops.split_weight(w).to(cuda),
+                                                         bias=b.to(cuda), act=3)))
     parity_log(f"[efficientnet] Swish epilogue: rel_max {r:.2e}")
 
 
@@ -133,7 +110,7 @@ def test_swish_epilogue_against_fp64(cuda):
 def test_im2col3_bitexact(cuda, H, W):
     """the generalised stem im2col at EfficientNet's 3x3 stride-2 adaptive padding, against F.pad + F.unfold"""
     n = 2
-    x = _images(n, H, W, seed=61)
+    x = images(n, H, W, seed=61)
     Ho, Wo = -(-H // 2), -(-W // 2)
     (pt, pb), (pl, pr) = adaptive_pad(H, 3, 2), adaptive_pad(W, 3, 2)
     cols = ops.im2col3(x.to(cuda), 3, 2, pt, pl, Ho, Wo, 32)
@@ -141,7 +118,7 @@ def test_im2col3_bitexact(cuda, H, W):
     L = u.shape[-1]
     assert L == Ho * Wo
     want = torch.cat([u.view(n, 3, 9, L).permute(0, 3, 2, 1).reshape(n * L, 27), torch.zeros(n * L, 5)], dim=1)
-    assert torch.equal(_bits(cols), _bits(ops.split_weight(want)))
+    assert torch.equal(bits(cols), bits(ops.split_weight(want)))
 
 
 # ------------------------------------------------------------------ 2. single blocks
@@ -163,7 +140,7 @@ def test_block_against_fp64(cuda, layer, block, what):
     out, _, ho, wo = CustomEfficientNet._block_cuda(p, x_cl, ops.to_split(x_cl), 2, h, w)
     cout = blk.linear_conv.conv.out_channels
     with torch.no_grad():
-        want = _f64(net).layers[layer][block](x.double()).permute(0, 2, 3, 1)
+        want = f64(net).layers[layer][block](x.double()).permute(0, 2, 3, 1)
     got = out.view(2, ho, wo, -1)
     assert bool((got[..., cout:] == 0).all()), "pad channels are not exactly 0"
     r = assert_close(got[..., :cout], want, 1e-3, f"block layers.{layer}.{block}")
@@ -174,9 +151,9 @@ def test_block_against_fp64(cuda, layer, block, what):
 # ------------------------------------------------------------------ 3. full size
 def test_b7_full_size_against_fp64(cuda):
     net = _b7(64, cuda)
-    x = _images(1, seed=65)
+    x = images(1, *HW, seed=65)
     outs = net(x.to(cuda))
-    ref = _f64(net, cuda)
+    ref = f64(net, cuda)
     gates = []
     hooks = [b.se.conv2.register_forward_hook(lambda m, i, o: gates.append(o.flatten().cpu()))
              for l in ref.layers[1:6] for b in l]
@@ -217,7 +194,7 @@ def test_secondfpn_kitti_levels_with_attached_twins_against_fp64(cuda):
     y = net(dev)[0]
     assert y.shape == (n, 640, 24, 80)
     with torch.no_grad():
-        want = _neck64(net)([t.double() for t in levels])[0]
+        want = f64(net)([t.double() for t in levels])[0]
     r = assert_close(y, want, 1e-3, "SECONDFPN KITTI levels")
     parity_log(f"[efficientnet] SECONDFPN at the KITTI levels: rel_max {r:.2e}")
     dev[0].mul_(0.5)
@@ -228,24 +205,14 @@ def test_secondfpn_kitti_levels_with_attached_twins_against_fp64(cuda):
 def test_images_to_view_transformer(cuda):
     """images -> B7 -> SECONDFPN -> view transformer built from the unmodified KITTI config, against the same chain in
     float64 (oracle.port lift / pooling), gated as test_gpu_image_encoder.py::test_images_to_view_transformer"""
-    from oracle import port
     cfg = json.load(open(os.path.join(GOLDEN, "image_encoder_cfg_kitti.json")))
-    backbone, neck = BACKBONES.build(cfg["img_backbone"]), NECKS.build(cfg["img_neck"])
-    backbone.eval()
-    neck.eval()
+    backbone, neck = BACKBONES.build(cfg["img_backbone"]).eval(), NECKS.build(cfg["img_neck"]).eval()
     backbone.load_state_dict(synth.make_efficientnet_state("b7", seed=68, out_indices=OUTS), strict=True)
     neck.load_state_dict(synth.make_secondfpn_state(seed=69, out_hw=(6, 20), **FPN), strict=True)
-    vt = NECKS.build(json.load(open(os.path.join(GOLDEN, "model_cfg_kitti.json")))["img_view_transformer"])
-    B, N, cin, mid, ctx, D, cam = 1, 1, 640, 640, 128, 112, 33
-    sd = synth.make_depthnet_state(cin, mid, ctx, D, cam, seed=70)
-    cams = synth.workload_cameras("kitti", B)
-    mlp = vt.get_mlp_input(cams["rots"], cams["trans"], cams["intrins"], cams["post_rots"], cams["post_trans"],
-                           cams["bda"])
-    sd["bn.running_mean"] = mlp.reshape(-1, cam).mean(0)
-    sd["bn.running_var"] = mlp.reshape(-1, cam).var(0, unbiased=False) + 1.0
-    vt.depth_net.load_state_dict(sd, strict=True)
-    backbone, neck, vt = backbone.to(cuda), neck.to(cuda), vt.to(cuda).eval()
-    imgs = _images(B * N, seed=71)
+    B, N = 1, 1
+    vt, cams, mlp = config_view_transformer("kitti", 70, B)
+    backbone, neck, vt = backbone.to(cuda), neck.to(cuda), vt.to(cuda)
+    imgs = images(B * N, *HW, seed=71)
 
     feat = neck(backbone(imgs.to(cuda)))[0]
     _, C, H, W = feat.shape
@@ -255,30 +222,9 @@ def test_images_to_view_transformer(cuda):
     bev, prob = vt(inp + [mlp.to(cuda)])
 
     with torch.no_grad():
-        stages = _f64(backbone, cuda)._forward_torch(imgs.double().to(cuda))
-        f64 = _neck64(neck)([s.cpu() for s in stages])[0]
-        dn = DepthNet(cin, mid, ctx, D, cam_channels=cam).eval()
-        dn.load_state_dict({k: v.cpu() for k, v in vt.depth_net.state_dict().items()})
-        out = dn.double()(f64, mlp.double())
-    vol, want_prob = port.lift(out[:, :D], out[:, D:D + ctx], B, N)
-    gc = vt.grid_config
-    frustum = port.create_frustum(vt.data_config["input_size"], vt.downsample, gc["dbound"])
-    geom = port.get_geometry(frustum, **cams)
-    X, Y, Z = vt.grid_size()
-    vox = ops._workspace(geom.numel() // 3, B, X, Y, Z, cuda).vox_id.cpu().long()
-    rows, keep = vol.reshape(-1, ctx), vox >= 0
-    want = torch.zeros(B * X * Y * Z, ctx, dtype=torch.float64).index_add_(0, vox[keep], rows[keep])
-    want = want.view(B, X, Y, Z, ctx)
-    rp = assert_close(prob, want_prob, 1e-3, "KITTI images -> view transformer: depth_prob")
-    got = bev.permute(0, 2, 3, 4, 1).reshape(-1, ctx).double().cpu()
-    scale = torch.zeros(B * X * Y * Z, ctx, dtype=torch.float64).index_add_(0, vox[keep], rows[keep].abs())
-    scale = scale + 1e-3 * float(want.abs().max())
-    worst = float(((got - want.reshape(-1, ctx)).abs() / scale).max())
-    assert worst <= 1e-2, f"pooled grid: a voxel off by {worst:.2e} of the magnitude of its terms"
-    rg = rel_err(got, want.reshape(-1, ctx))
-    assert rg <= 1e-3, f"pooled grid: rel_max {rg:.2e}"
-    parity_log(f"[efficientnet] KITTI images -> view transformer: depth_prob rel_max {rp:.2e}, grid rel_max {rg:.2e}, "
-               f"worst voxel {worst:.2e} of its terms' magnitude")
+        stages = f64(backbone, cuda)._forward_torch(imgs.double().to(cuda))
+        out = f64(vt.depth_net)(f64(neck)([s.cpu() for s in stages])[0], mlp.double())
+    check_pooled(vt, cams, out, prob, bev, B, N, "[efficientnet] KITTI images -> view transformer", "terms")
 
 
 def test_golden_on_gpu(cuda):
@@ -294,16 +240,7 @@ def test_golden_on_gpu(cuda):
 
 # ------------------------------------------------------------------ 4. only library kernels, graph-safe
 def test_only_library_kernels_and_cuda_graph(cuda):
-    """tests/efficientnet_trace.py in a process of its own (see test_gpu_depthnet.py)"""
-    here = os.path.dirname(os.path.abspath(__file__))
-    flags = ["-s"] if sys.flags.no_user_site else []
-    r = subprocess.run([sys.executable, *flags, os.path.join(here, "efficientnet_trace.py")], capture_output=True,
-                       text=True, timeout=1200)
-    assert r.returncode == 0, f"efficientnet_trace.py failed:\n{r.stdout}\n{r.stderr}"
-    res = json.loads(r.stdout.strip().splitlines()[-1])
-    print(f"[efficientnet launches] counted {res['counted']}, trace: {res['kernels']} occ:: kernels + "
-          f"{res['memsets']} memsets")
-    assert not res["other"], f"non-library GPU work: {res['other'][:5]}"
+    res = run_trace("b7", 1200)
     assert res["memsets"] == 0
     # stem im2col + GEMM; 55 blocks x (depthwise + SE gate + SE scale + linear GEMM) + 51 expand GEMMs (layers.1 has
     # none) + 52 splits (after every block followed by an expand conv or by layers.6); layers.6 GEMM + split;
@@ -316,20 +253,20 @@ def test_only_library_kernels_and_cuda_graph(cuda):
 def test_shape_contract(cuda):
     net = CustomEfficientNet("b0", out_indices=(2, 3)).eval().to(cuda)
     with pytest.raises(RuntimeError, match="multiples of 32"):
-        net(_images(1, 100, 128).to(cuda))
-    assert net.cpu()(_images(1, 100, 128))[1].shape == (1, 40, 13, 16)  # the CPU forward still runs
+        net(images(1, 100, 128).to(cuda))
+    assert net.cpu()(images(1, 100, 128))[1].shape == (1, 40, 13, 16)  # the CPU forward still runs
     net = net.to(cuda).train()
     with pytest.raises(RuntimeError, match="eval mode"):
-        net(_images(1, 64, 64).to(cuda))
+        net(images(1, 64, 64).to(cuda))
 
 
 def test_bf16_mode(cuda):
     net, neck = _b7(72, cuda), _neck(73, cuda)
-    x = _images(1, seed=74)
+    x = images(1, *HW, seed=74)
     with ops.precision("bf16"):
         y = neck(list(net(x.to(cuda))))[0]
     with torch.no_grad():
-        want = _neck64(neck)([s.cpu() for s in _f64(net, cuda)._forward_torch(x.double().to(cuda))])[0]
+        want = f64(neck)([s.cpu() for s in f64(net, cuda)._forward_torch(x.double().to(cuda))])[0]
     # single-pass bf16 operands (~3e-3 per contraction) through 112 GEMMs and the FPN, a mode without a reference twin:
     # bounded by its max and rms error (9.7e-3 / 3.9e-3 measured on H100)
     r, q = rel_err(y, want), rel_rms(y, want)

@@ -5,14 +5,13 @@ oracle is image_encoder.py's torch forward on the host in float64 (pinned to tor
 SECONDFPN by tests/test_cpu_image_encoder.py)."""
 import json
 import os
-import subprocess
-import sys
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from util import GOLDEN, assert_close, parity_log, rel_err, rel_rms
+from util import GOLDEN, assert_close, bits, f64, images, parity_log, rel_err, rel_rms, run_trace
+from vt_chain import check_pooled, config_view_transformer
 from occformer_b200 import BACKBONES, NECKS, ops, synth
 from occformer_b200.common import attach_twin, twin_of
 from occformer_b200.depthnet import DepthNet
@@ -23,10 +22,7 @@ pytestmark = pytest.mark.gpu
 KERNEL_TOL = 5e-5
 SENTINEL = -1234.5
 FPN = dict(in_channels=[256, 512, 1024, 2048], out_channels=[128, 128, 128, 128], upsample_strides=[0.25, 0.5, 1, 2])
-
-
-def _bits(t):
-    return t.detach().contiguous().view(torch.int32).cpu()
+HW = (256, 704)
 
 
 def _backbone(seed, dev):
@@ -41,37 +37,20 @@ def _neck(seed, dev, cfg=FPN):
     return net.to(dev)
 
 
-def _backbone64(net):
-    """the same module on the host in float64 (the oracle); likewise _neck64"""
-    ref = ResNet(50, out_indices=net.out_indices).eval()
-    ref.load_state_dict({k: v.cpu() for k, v in net.state_dict().items()})
-    return ref.double()
-
-
-def _neck64(net):
-    ref = SECONDFPN(net.in_channels, net.out_channels, net.upsample_strides).eval()
-    ref.load_state_dict({k: v.cpu() for k, v in net.state_dict().items()})
-    return ref.double()
-
-
-def _images(n, H=256, W=704, seed=0):
-    return torch.randn(n, 3, H, W, generator=torch.Generator().manual_seed(seed))
-
-
 # ------------------------------------------------------------------ 1. the new kernels, one launch at a time
 @pytest.mark.parametrize("H,W", [(256, 704), (37, 50), (8, 9)])
 def test_stem_im2col_bitexact(cuda, H, W):
     """against F.unfold reordered to (ky, kx, c) columns, padded to 160 with zeros and split by split_weight: the image
     borders (zero padding) and the zero pad columns included"""
     n = 2
-    x = _images(n, H, W, seed=1)
+    x = images(n, H, W, seed=1)
     cols = ops.stem_im2col(x.to(cuda))
     u = F.unfold(x, 7, padding=3, stride=2)  # (n, c*49 + ky*7 + kx, L)
     L = u.shape[-1]
     want = u.view(n, 3, 49, L).permute(0, 3, 2, 1).reshape(n * L, 147)
     want = torch.cat([want, torch.zeros(n * L, 13)], dim=1)
     assert cols.shape == (n * ((H - 1) // 2 + 1) * ((W - 1) // 2 + 1), 160) == want.shape
-    assert torch.equal(_bits(cols), _bits(ops.split_weight(want)))
+    assert torch.equal(bits(cols), bits(ops.split_weight(want)))
 
 
 @pytest.mark.parametrize("H,W,C", [(128, 352, 64), (15, 22, 96), (1, 3, 32)])
@@ -84,7 +63,7 @@ def test_maxpool_bitexact(cuda, H, W, C):
     got = ops.maxpool3x3s2(x.permute(0, 2, 3, 1).contiguous().to(cuda))
     want = F.max_pool2d(x, 3, 2, 1).permute(0, 2, 3, 1).contiguous()
     assert got.shape == want.shape
-    assert torch.equal(_bits(got).view(-1, C), _bits(ops.split_weight(want.view(-1, C))))
+    assert torch.equal(bits(got).view(-1, C), bits(ops.split_weight(want.view(-1, C))))
     if H > 2:
         assert bool((want[:, 0] < 0).any())  # a border window whose maximum is negative
 
@@ -95,7 +74,7 @@ def test_space_to_depth_bitexact(cuda, f):
     x = ops.to_split(torch.randn(n, H, W, C, generator=torch.Generator().manual_seed(3)).to(cuda))
     got = ops.space_to_depth(x, f)
     want = x.cpu().view(n, H // f, f, W // f, f, C).permute(0, 1, 3, 2, 4, 5).reshape(n, H // f, W // f, f * f * C)
-    assert torch.equal(_bits(got), _bits(want))
+    assert torch.equal(bits(got), bits(want))
 
 
 @pytest.mark.parametrize("f,C,ldo,off", [(2, 128, 512, 384), (2, 64, 200, 8), (4, 32, 96, 32)])
@@ -105,9 +84,9 @@ def test_depth_to_space_bitexact(cuda, f, C, ldo, off):
     out = torch.full((n * h * w * f * f, ldo), SENTINEL, device=cuda)
     ops.depth_to_space_into(y, n, h, w, f, out, off)
     want = y.cpu().view(n, h, w, f, f, C).permute(0, 1, 3, 2, 4, 5).reshape(-1, C)
-    assert torch.equal(_bits(out[:, off:off + C]), _bits(want))
+    assert torch.equal(bits(out[:, off:off + C]), bits(want))
     outside = torch.cat([out[:, :off], out[:, off + C:]], dim=1)
-    assert bool((_bits(outside) == _bits(torch.tensor(SENTINEL))).all()), "columns outside the slice changed"
+    assert bool((bits(outside) == bits(torch.tensor(SENTINEL))).all()), "columns outside the slice changed"
 
 
 # ------------------------------------------------------------------ 2. the 2-D stride-2 conv (Z = KZ = 1)
@@ -139,24 +118,24 @@ def test_bottleneck_against_fp64(cuda, layer, block):
     x = torch.randn(4, cin, 32, 88, generator=torch.Generator().manual_seed(7)).abs()
     x_cl = x.permute(0, 2, 3, 1).contiguous().to(cuda).unsqueeze(3)
     out, out_s = ResNet._bottleneck_cuda(net._prepare()["blocks"][idx], x_cl, ops.to_split(x_cl))
-    ref = _backbone64(net)
+    ref = f64(net)
     with torch.no_grad():
         want = getattr(ref, layer)[block](x.double()).permute(0, 2, 3, 1)
     r = assert_close(out[:, :, :, 0], want, 1e-3, f"Bottleneck {layer}.{block}")
-    assert torch.equal(_bits(out_s), _bits(ops.to_split(out)))
+    assert torch.equal(bits(out_s), bits(ops.to_split(out)))
     parity_log(f"[image encoder] Bottleneck {layer}.{block}: rel_max {r:.2e}")
 
 
 def test_resnet50_against_fp64(cuda):
     net = _backbone(8, cuda)
-    x = _images(6, seed=9)
+    x = images(6, *HW, seed=9)
     outs = net(x.to(cuda))
     with torch.no_grad():
-        want = _backbone64(net)(x.double())
+        want = f64(net)(x.double())
     assert len(outs) == 4
     for i, (o, w) in enumerate(zip(outs, want)):
         assert o.shape == w.shape and o.is_contiguous(memory_format=torch.channels_last)
-        assert torch.equal(_bits(twin_of(o)), _bits(ops.to_split(o.permute(0, 2, 3, 1).contiguous())))
+        assert torch.equal(bits(twin_of(o)), bits(ops.to_split(o.permute(0, 2, 3, 1).contiguous())))
         r = assert_close(o, w, 1e-3, f"ResNet-50 stage {i}")
         pos = float((w > 0).double().mean())
         assert 0.05 < pos < 0.95, f"stage {i}: {pos:.1%} positive activations -- a vacuous comparison"
@@ -186,7 +165,7 @@ def test_secondfpn_against_fp64(cuda, twin):
     y = out[0]
     assert y.shape == (n, 512, 16, 44) and y.is_contiguous(memory_format=torch.channels_last)
     with torch.no_grad():
-        want = _neck64(net)([t.double() for t in levels])[0]
+        want = f64(net)([t.double() for t in levels])[0]
     r = assert_close(y, want, 1e-3, f"SECONDFPN R50 twin={twin}")
     parity_log(f"[image encoder] SECONDFPN R50 (twin={twin if isinstance(twin, str) else int(twin)}): rel_max {r:.2e}")
 
@@ -202,10 +181,8 @@ def test_secondfpn_other_strides(cuda):
         levels = [torch.randn(2, c, int(8 / s), int(12 / s), generator=g) for c, s in
                   zip(cfg["in_channels"], cfg["upsample_strides"])]
         y = net([t.to(cuda) for t in levels])[0]
-        ref = SECONDFPN(**cfg).eval()
-        ref.load_state_dict({k: v.cpu() for k, v in net.state_dict().items()})
         with torch.no_grad():
-            want = ref.double()([t.double() for t in levels])[0]
+            want = f64(net)([t.double() for t in levels])[0]
         assert_close(y, want, 1e-3, f"SECONDFPN {cfg}")
 
 
@@ -214,22 +191,14 @@ def test_images_to_view_transformer(cuda):
     """images -> ResNet -> SECONDFPN -> the reference glue's x.view(B, N, C, H, W) -> the view transformer built from the
     unmodified nuScenes R50 config, against the same chain on the host (torch modules in float64, oracle.port lift /
     voxel pooling) as test_gpu_depthnet.py::test_view_transformer_from_config"""
-    from oracle import port
     cfg = json.load(open(os.path.join(GOLDEN, "image_encoder_cfg_nusc.json")))
     backbone, neck = BACKBONES.build(cfg["img_backbone"]).eval(), NECKS.build(cfg["img_neck"]).eval()
     backbone.load_state_dict(synth.make_resnet_state(14), strict=True)
     neck.load_state_dict(synth.make_secondfpn_state(seed=15, **FPN), strict=True)
-    vt = NECKS.build(json.load(open(os.path.join(GOLDEN, "model_cfg_nusc_r50.json")))["img_view_transformer"])
-    B, N, cin, mid, ctx, D, cam = 1, 6, 512, 512, 128, 112, 27
-    sd = synth.make_depthnet_state(cin, mid, ctx, D, cam, seed=16)
-    cams = synth.workload_cameras("nusc_ref", B)
-    mlp = vt.get_mlp_input(cams["rots"], cams["trans"], cams["intrins"], cams["post_rots"], cams["post_trans"],
-                           cams["bda"])
-    sd["bn.running_mean"] = mlp.reshape(-1, cam).mean(0)
-    sd["bn.running_var"] = mlp.reshape(-1, cam).var(0, unbiased=False) + 1.0
-    vt.depth_net.load_state_dict(sd, strict=True)
-    backbone, neck, vt = backbone.to(cuda), neck.to(cuda), vt.to(cuda).eval()
-    imgs = _images(B * N, seed=17)
+    B, N = 1, 6
+    vt, cams, mlp = config_view_transformer("nusc_r50", 16, B)
+    backbone, neck, vt = backbone.to(cuda), neck.to(cuda), vt.to(cuda)
+    imgs = images(B * N, *HW, seed=17)
 
     feat = neck(backbone(imgs.to(cuda)))[0]
     _, C, H, W = feat.shape
@@ -238,35 +207,9 @@ def test_images_to_view_transformer(cuda):
     bev, prob = vt(inp + [mlp.to(cuda)])
 
     with torch.no_grad():
-        f64 = _neck64(neck)(list(_backbone64(backbone)(imgs.double())))[0]
-        dn = DepthNet(cin, mid, ctx, D, cam_channels=cam).eval()
-        dn.load_state_dict({k: v.cpu() for k, v in vt.depth_net.state_dict().items()})
-        out = dn.double()(f64, mlp.double())
-    vol, want_prob = port.lift(out[:, :D], out[:, D:D + ctx], B, N)
-    gc = vt.grid_config
-    frustum = port.create_frustum(vt.data_config["input_size"], vt.downsample, gc["dbound"])
-    geom = port.get_geometry(frustum, **cams)
-    # pooled over the kernel's own voxel assignment (see test_view_transformer_from_config)
-    X, Y, Z = vt.grid_size()
-    vox = ops._workspace(geom.numel() // 3, B, X, Y, Z, cuda).vox_id.cpu().long()
-    rows, keep = vol.reshape(-1, ctx), vox >= 0
-    want = torch.zeros(B * X * Y * Z, ctx, dtype=torch.float64).index_add_(0, vox[keep], rows[keep])
-    want = want.view(B, X, Y, Z, ctx)
-    rp = assert_close(prob, want_prob, 1e-3, "images -> view transformer: depth_prob")
-    # The grid within 1e-3 of its largest value.  A voxel is a sum of up to hundreds of signed point terms prob * feature,
-    # so its error scales with the sum of their magnitudes, not with its value (a few voxels cancel to near zero); and a
-    # softmax probability carries the absolute error of its logit as a relative one (1e-4 of logits of magnitude tens):
-    # every voxel within 1e-2 of the magnitude of its terms (2.1e-3 measured), with a floor of 1e-6 of the grid's
-    # largest value (points of a vanishing depth probability are fp32 denormals)
-    got = bev.permute(0, 2, 3, 4, 1).reshape(-1, ctx).double().cpu()
-    scale = torch.zeros(B * X * Y * Z, ctx, dtype=torch.float64).index_add_(0, vox[keep], rows[keep].abs())
-    scale = scale + 1e-3 * float(want.abs().max())
-    worst = float(((got - want.reshape(-1, ctx)).abs() / scale).max())
-    assert worst <= 1e-2, f"pooled grid: a voxel off by {worst:.2e} of the magnitude of its terms"
-    rg = rel_err(got, want.reshape(-1, ctx))
-    assert rg <= 1e-3, f"pooled grid: rel_max {rg:.2e}"
-    parity_log(f"[image encoder] images -> view transformer: depth_prob rel_max {rp:.2e}, grid rel_max {rg:.2e}, "
-               f"worst voxel {worst:.2e} of its terms' magnitude")
+        out = f64(vt.depth_net)(f64(neck)(list(f64(backbone)(imgs.double())))[0], mlp.double())
+    # every voxel within 1e-2 of the magnitude of its terms: 2.1e-3 measured on H100
+    check_pooled(vt, cams, out, prob, bev, B, N, "[image encoder] images -> view transformer", "terms")
 
 
 def test_depthnet_on_channels_last_map_is_bitwise_nchw(cuda):
@@ -279,21 +222,12 @@ def test_depthnet_on_channels_last_map_is_bitwise_nchw(cuda):
     mlp = torch.randn(1, 6, cam, generator=g).to(cuda)
     x_cl = x.contiguous(memory_format=torch.channels_last)
     assert not x_cl.is_contiguous()
-    assert torch.equal(_bits(net(x_cl, mlp)), _bits(net(x, mlp)))
+    assert torch.equal(bits(net(x_cl, mlp)), bits(net(x, mlp)))
 
 
 # ------------------------------------------------------------------ 5. only library kernels, graph-safe
 def test_only_library_kernels_and_cuda_graph(cuda):
-    """tests/image_encoder_trace.py in a process of its own (see test_gpu_depthnet.py)"""
-    here = os.path.dirname(os.path.abspath(__file__))
-    flags = ["-s"] if sys.flags.no_user_site else []
-    r = subprocess.run([sys.executable, *flags, os.path.join(here, "image_encoder_trace.py")], capture_output=True,
-                       text=True, timeout=900)
-    assert r.returncode == 0, f"image_encoder_trace.py failed:\n{r.stdout}\n{r.stderr}"
-    res = json.loads(r.stdout.strip().splitlines()[-1])
-    print(f"[image encoder launches] counted {res['counted']}, trace: {res['kernels']} occ:: kernels + "
-          f"{res['memsets']} memsets")
-    assert not res["other"], f"non-library GPU work: {res['other'][:5]}"
+    res = run_trace("r50", 900)
     # stem im2col + GEMM + max-pool, 16 Bottlenecks x (3 convs + split) + 4 downsamples, SECONDFPN: 2 space_to_depth +
     # 3 convs + GEMM + depth_to_space
     assert res["counted"] == res["kernels"] + res["memsets"] == 3 + 16 * 4 + 4 + 7
@@ -303,14 +237,14 @@ def test_only_library_kernels_and_cuda_graph(cuda):
 # ------------------------------------------------------------------ 6. shape contract, bf16 mode
 def test_shape_contract(cuda):
     net = _backbone(20, cuda)
-    x = _images(1, 100, 128, seed=21)
+    x = images(1, 100, 128, seed=21)
     with pytest.raises(RuntimeError, match="multiples of 32"):
         net(x.to(cuda))
     y = net.cpu()(x)  # the CPU forward still runs
     assert y[3].shape == (1, 2048, 4, 4)
     net = net.to(cuda).train()
     with pytest.raises(RuntimeError, match="eval mode"):
-        net(_images(1, 64, 64).to(cuda))
+        net(images(1, 64, 64).to(cuda))
     neck = _neck(22, cuda)
     with pytest.raises(RuntimeError, match="one output size"):
         neck([torch.rand(1, c, 16, 16, device=cuda) for c in FPN["in_channels"]])
@@ -326,11 +260,11 @@ def test_shape_contract(cuda):
 
 def test_bf16_mode(cuda):
     backbone, neck = _backbone(23, cuda), _neck(24, cuda)
-    x = _images(6, seed=25)
+    x = images(6, *HW, seed=25)
     with ops.precision("bf16"):
         y = neck(list(backbone(x.to(cuda))))[0]
     with torch.no_grad():
-        want = _neck64(neck)(list(_backbone64(backbone)(x.double())))[0]
+        want = f64(neck)(list(f64(backbone)(x.double())))[0]
     # single-pass bf16 operands (~3e-3 per contraction) through 53 stacked convs and the FPN, a mode without a reference
     # twin: bounded by its max and rms error (5.5e-2 / 3.5e-2 measured on H100)
     r, q = rel_err(y, want), rel_rms(y, want)

@@ -4,8 +4,8 @@ head simple_test) under torch.profiler.  Every kernel of the library lives in na
 occ:: kernels plus the memsets of the trace (torch issues none in this step)."""
 import pytest
 import torch
-from torch.profiler import ProfilerActivity, profile
 
+from util import trace
 from occformer_b200 import synth
 
 pytestmark = pytest.mark.gpu
@@ -51,18 +51,9 @@ def _pr1_step(cuda):
 
 
 def test_launch_count_matches_profiler_trace(cuda):
-    from occformer_b200 import ops
     step = _pr1_step(cuda)
     step()  # warm-up: lazy weight packing, workspaces, module loading
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        n0 = ops.LAUNCH_COUNT[0]
-        step()
-        torch.cuda.synchronize()
-        counted = ops.LAUNCH_COUNT[0] - n0
-    gpu = [e.name for e in prof.events() if str(e.device_type).endswith("CUDA")]
-    kernels = sum("occ::" in n for n in gpu)
-    memsets = sum(n.startswith("Memset") for n in gpu)
-    print(f"[launch count] counted {counted}, trace: {kernels} occ:: kernels + {memsets} memsets")
-    assert kernels > 0 and memsets > 0
-    assert counted == kernels + memsets
+    t = trace(step)
+    print(f"[launch count] counted {t['counted']}, trace: {t['kernels']} occ:: kernels + {t['memsets']} memsets")
+    assert t["kernels"] > 0 and t["memsets"] > 0
+    assert t["counted"] == t["kernels"] + t["memsets"]

@@ -1,9 +1,14 @@
+import copy
+import json
 import os
+import subprocess
+import sys
 
 import numpy as np
 import torch
 
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+HERE = os.path.dirname(os.path.abspath(__file__))
+GOLDEN = os.path.join(HERE, "golden")
 
 # north_star tolerance: 1e-3 relative fp32 per output tensor (SURVEY.md 8(d))
 RTOL = 1e-3
@@ -62,6 +67,51 @@ def round_tf32(t):
     i = t.clone().contiguous().view(torch.int32)
     i.add_(0x1000).bitwise_and_(-8192)
     return i.view(torch.float32)
+
+
+def bits(t):
+    return t.detach().contiguous().view(torch.int32).cpu()
+
+
+def images(n, H, W, seed=0):
+    return torch.randn(n, 3, H, W, generator=torch.Generator().manual_seed(seed))
+
+
+def f64(net, device=None):
+    """The same module in float64 in eval mode (the oracle of the GPU tests), on the host, or on `device` when given.
+    .cpu() drops the prepared-parameter cache, so the copy carries no CUDA state."""
+    ref = copy.deepcopy(net).cpu().double().eval()
+    return ref if device is None else ref.to(device)
+
+
+def trace(fn):
+    """One call of fn under torch.profiler -> dict(counted: the library's launch count over the call (ops.LAUNCH_COUNT),
+    kernels / memsets: the occ:: kernels and memsets of the trace, other: the names of any other GPU work)"""
+    from torch.profiler import ProfilerActivity, profile
+    from occformer_b200 import ops
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        n0 = ops.LAUNCH_COUNT[0]
+        fn()
+        torch.cuda.synchronize()
+        counted = ops.LAUNCH_COUNT[0] - n0
+    gpu = [e.name for e in prof.events() if str(e.device_type).endswith("CUDA")]
+    return dict(counted=counted, kernels=sum("occ::" in e for e in gpu), memsets=sum(e.startswith("Memset") for e in gpu),
+                other=sorted({e for e in gpu if "occ::" not in e and not e.startswith("Memset")}))
+
+
+def run_trace(case, timeout):
+    """tests/forward_trace.py <case> in a process of its own, with this interpreter's settings: its profiler session and
+    graph capture must not change what a later profiler session of this process records (test_gpu_launch_count compares
+    a trace with the launch counter).  Asserts that the forward ran only library kernels and memsets.  -> its result"""
+    flags = ["-s"] if sys.flags.no_user_site else []
+    r = subprocess.run([sys.executable, *flags, os.path.join(HERE, "forward_trace.py"), case], capture_output=True,
+                       text=True, timeout=timeout)
+    assert r.returncode == 0, f"forward_trace.py {case} failed:\n{r.stdout}\n{r.stderr}"
+    res = json.loads(r.stdout.strip().splitlines()[-1])
+    print(f"[{case} launches] counted {res['counted']}, trace: {res['kernels']} occ:: kernels + {res['memsets']} memsets")
+    assert not res["other"], f"non-library GPU work: {res['other'][:5]}"
+    return res
 
 
 class FakeLibrary:
