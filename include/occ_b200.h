@@ -240,7 +240,9 @@ int occ_se_scale(const float* y, const float* gate, float* out, int n, int rows_
  * win_shift < 0: tokn rows in token order;  win_shift = 0 / 1 (needs X, XY % X == 0): tokn in the WINDOW LAYOUT of the
  * un-shifted / shifted 7x7 partition -- token (img, x, y) at row window*64 + t with window = (wx*nWy + wy)*n_images + img,
  * occ_window_layout_rows() rows in total,
- * zero-initialised once by the caller (pad positions are never written) -- the operand of occ_swin_qkv_attention. */
+ * zero-initialised once by the caller (pad positions are never written) -- the operand of occ_swin_qkv_attention.
+ * Limits: C in {128, 256, 512, 1024}, Z <= 16, groups <= 32 with C / groups a multiple of 4, and the Z-column buffer
+ * Z * C * 4 bytes of one (b, x, y) column within 48 KiB (C = 1024 needs Z <= 12); -1 / -2 otherwise, nothing enqueued. */
 int occ_gn_relu_zmean_ln(const float* y, const double* stats, const float* gn_w, const float* gn_b,
                          const float* ln_w, const float* ln_b, float* tok, float* tokn, int B, int XY, int Z, int C,
                          int groups, int X, int win_shift, occ_stream_t stream);
@@ -252,13 +254,16 @@ int occ_layernorm(const float* in, const float* w, const float* b, float* out, l
 int occ_gn_apply(const float* in, const double* stats, const float* w, const float* b, const float* residual,
                  float* out, float* out_split, long long rows, int rows_per_batch, int C, int groups, int ldo,
                  int out_off, int relu, occ_stream_t stream);
-/* ASPP image-pooling branch: GAP -> 1x1 conv -> GN -> ReLU -> broadcast (aspp.py:89-95,113-114).
- * sums_ws: workspace of B*ch doubles followed by B*ch floats. */
+/* ASPP image-pooling branch: GAP -> 1x1 conv -> GN -> ReLU -> broadcast (aspp.py:89-95,113-114) into columns
+ * [out_off, out_off + ch) of the S32 concat buffer cat (rows of ldo floats; ldo, out_off multiples of 32,
+ * out_off + ch <= ldo); ch % 32 == 0, ch <= 1024, 256 % (ch / 4) == 0, B <= 65535.
+ * sums_ws: workspace of B*ch doubles followed by B*ch floats.  The column sums are fp64 atomics: not bit-reproducible. */
 int occ_aspp_gap_branch(const float* in, double* sums_ws, const float* wconv, const float* gw, const float* gb,
                         float* cat, int B, int rows_per_batch, int ch, int groups, int ldo, int out_off,
                         occ_stream_t stream);
 /* coeff = sigmoid(<x,w>+b); out = x + coeff * bev + identity (identity optionally GroupNorm'd: strided skip path)
- * dualpath_block.py:36-41,79-82 */
+ * dualpath_block.py:36-41,79-82.  x / identity / out rows are voxel tokens, bev (B*XY, C) one row per (b, x, y) column.
+ * C in {128, 256, 512, 1024} (-2 otherwise, nothing enqueued); with id_stats, C / groups a multiple of 4. */
 int occ_dualpath_fuse(const float* x, const float* bev, const float* cw, float cbias, const float* identity,
                       int identity_split /*identity is S32*/, const double* id_stats, const float* id_w,
                       const float* id_b, int groups, float* out /*fp32, optional*/, float* out_split /*S32, optional*/,

@@ -32,10 +32,17 @@ __device__ __forceinline__ void gn_mean_rstd(const double* __restrict__ stats, i
   *rstd = (float)(1.0 / sqrt(var + (double)kEps));
 }
 
-// LayerNorm of a row held as NV float4 per lane (C = 128*NV).  two-pass in registers.
+// LayerNorm of a row held as NV float4 per lane (C = 128*NV).  two-pass in registers, on the row shifted by its first
+// element: for a row whose offset dwarfs its spread the shifted values are exact and small, so the fp32 sums lose no
+// digits to the offset (an unshifted sum of values near 1e3 puts ~1e-5 of the spread into the mean).
 template <int NV>
 __device__ __forceinline__ void warp_layernorm(float4 (&v)[NV], int C, const float* __restrict__ gamma,
                                                const float* __restrict__ beta, int lane) {
+  const float shift = __shfl_sync(0xffffffffu, v[0].x, 0);
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    v[i].x -= shift; v[i].y -= shift; v[i].z -= shift; v[i].w -= shift;
+  }
   float s = 0.f;
 #pragma unroll
   for (int i = 0; i < NV; ++i) s += v[i].x + v[i].y + v[i].z + v[i].w;
@@ -188,14 +195,15 @@ layernorm_generic_kernel(const float* __restrict__ in, const float* __restrict__
   const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= rows) return;
   const float* src = in + row * C;
+  const float shift = src[0];  // as warp_layernorm: the sums run on the row shifted by its first element
   float s = 0.f;
-  for (int c = lane; c < C; c += 32) s += src[c];
+  for (int c = lane; c < C; c += 32) s += src[c] - shift;
   const float mean = warp_sum(s) / (float)C;
   float q = 0.f;
-  for (int c = lane; c < C; c += 32) { const float d = src[c] - mean; q += d * d; }
+  for (int c = lane; c < C; c += 32) { const float d = (src[c] - shift) - mean; q += d * d; }
   const float rstd = rsqrtf(warp_sum(q) / (float)C + kEps);
   for (int c = lane; c < C; c += 32) {  // split: C % 32 == 0, lanes (2t, 2t+1) form packed word t of the chunk
-    const float o = (src[c] - mean) * rstd * w[c] + b[c];
+    const float o = ((src[c] - shift) - mean) * rstd * w[c] + b[c];
     if (split) {
       const float o2 = __shfl_xor_sync(0xffffffffu, o, 1);
       if (!(lane & 1)) {
@@ -515,6 +523,19 @@ using namespace occ;
     default: return OCC_EUNSUPPORTED;            \
   }
 
+// Static shared memory of gn_relu_zmean_ln_kernel (s_mean, s_rstd).  Without an opt-in, static + dynamic shared memory
+// must stay within 48 KiB, so a Z-column buffer above 44 KiB (C = 1024 at Z = 6 or 12) needs the attribute raised.
+constexpr size_t kZmeanStaticSmem = 2 * 16 * 32 * sizeof(float);
+
+template <int NV, int R, typename... Args>
+static int launch_gn_relu_zmean_ln(int blocks, int threads, size_t smem, cudaStream_t stream, Args... args) {
+  auto* kernel = gn_relu_zmean_ln_kernel<NV, R>;
+  if (smem + kZmeanStaticSmem > 48 * 1024) OCC_ENSURE_SMEM(kernel, smem);
+  kernel<<<blocks, threads, smem, stream>>>(args...);
+  OCC_LAUNCH_CHECK();
+  return OCC_OK;
+}
+
 extern "C" int occ_gn_relu_zmean_ln(const float* y, const double* stats, const float* gn_w, const float* gn_b,
                                     const float* ln_w, const float* ln_b, float* tok, float* tokn, int B, int XY,
                                     int Z, int C, int groups, int X, int win_shift, cudaStream_t stream) {
@@ -540,15 +561,13 @@ extern "C" int occ_gn_relu_zmean_ln(const float* y, const double* stats, const f
   const int blocks = (int)((ncols + cols - 1) / cols);
   const int threads = cols * wpc * 32;
   OCC_REQUIRE(threads <= 512);
-  if (R == 4) {
-    gn_relu_zmean_ln_kernel<1, 4><<<blocks, threads, smem, stream>>>(y, stats, gn_w, gn_b, ln_w, ln_b, tok, tokn, B, XY, Z,
-                                                                     C, groups, cols, wg, wl);
-  } else {
-    DISPATCH_NV(C, (gn_relu_zmean_ln_kernel<NV, 1><<<blocks, threads, smem, stream>>>(y, stats, gn_w, gn_b, ln_w, ln_b, tok,
-                                                                                    tokn, B, XY, Z, C, groups, cols, wg, wl)));
-  }
-  OCC_LAUNCH_CHECK();
-  return OCC_OK;
+  if (R == 4)
+    return launch_gn_relu_zmean_ln<1, 4>(blocks, threads, smem, stream, y, stats, gn_w, gn_b, ln_w, ln_b, tok, tokn, B, XY,
+                                         Z, C, groups, cols, wg, wl);
+  int rc = OCC_OK;
+  DISPATCH_NV(C, (rc = launch_gn_relu_zmean_ln<NV, 1>(blocks, threads, smem, stream, y, stats, gn_w, gn_b, ln_w, ln_b, tok,
+                                                      tokn, B, XY, Z, C, groups, cols, wg, wl)));
+  return rc;
 }
 
 extern "C" int occ_layernorm(const float* in, const float* w, const float* b, float* out, long long rows, int C,
@@ -591,8 +610,9 @@ extern "C" int occ_aspp_gap_branch(const float* in, double* sums_ws, const float
                                    const float* gb, float* cat, int B, int rows_per_batch, int ch, int groups, int ldo,
                                    int out_off, cudaStream_t stream) {
   OCC_REQUIRE(in && sums_ws && wconv && gw && gb && cat);
-  OCC_REQUIRE(B > 0 && rows_per_batch > 0 && ch % 32 == 0 && ch <= 1024 && groups > 0 && ch % groups == 0 && 256 % (ch / 4) == 0);
-  OCC_REQUIRE(ldo % 32 == 0 && out_off % 32 == 0);  // the branch lands in the S32 concat buffer
+  OCC_REQUIRE(B > 0 && B <= 65535 && rows_per_batch > 0 && ch % 32 == 0 && ch <= 1024 && groups > 0 && ch % groups == 0 &&
+              256 % (ch / 4) == 0);  // B is the colsum grid's y
+  OCC_REQUIRE(ldo % 32 == 0 && out_off % 32 == 0 && out_off + ch <= ldo);  // a slice of the S32 concat buffer
   OCC_MEMSET(sums_ws, 0, (size_t)B * ch * sizeof(double), stream);
   const int chunk = 256;
   dim3 grid((rows_per_batch + chunk - 1) / chunk, B);
