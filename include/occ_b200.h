@@ -300,18 +300,23 @@ int occ_swin_qkv_attention(const float* tokn, const float* wqkv, const float* bq
  * occ_conv_bf16x3. */
 /* [LayerNorm (norms.k of the encoder layer) of each row ->] out_f32 = x (fp32), out_s32 = x (S32), out_pos = x + pos[token]
  * (S32; pos (Nq, C) = SinePositionalEncoding3D + level_encoding of the token's level: query_pos of the reference); any of
- * the three outputs may be NULL; ln_w / ln_b NULL = no normalisation. */
+ * the three outputs may be NULL (not all three); ln_w / ln_b NULL = no normalisation, both or neither; out_pos needs pos.
+ * C % 32 == 0, 32 <= C <= 1024, C / 32 in {1, 2, 3, 4, 6, 8, 12, 16, 24, 32} (else -2); 1 <= L <= 4.  LayerNorm eps 1e-5,
+ * biased variance. */
 int occ_neck_token_prep(const float* in, const float* ln_w, const float* ln_b, const float* pos, float* out_f32,
                         float* out_s32, float* out_pos, int L, int B, const int* grids, int C, occ_stream_t stream);
 /* multi_scale_deformable_attn_pytorch + the sampling-location arithmetic of MultiScaleDeformableAttention3D.forward:
  * value (rows, value_ld) = value_proj output, head h at columns [h*head_ld, h*head_ld + E/H) (head_ld = E/H, or E/H
  * rounded up to 32 floats so that a head slice is one 128-byte line); ow (rows, H*L*P*4) = [sampling_offsets (h,l,p,(z,y,x)) | attention logits (h,l,p)];
  * out (rows, E) S32 = sum_{l,p} softmax(logits) * trilinear(value level l)(ref + offset / (Z_l,Y_l,X_l)), zeros outside,
- * align_corners=False; strides = the L feature strides (HOST floats; reference-point arithmetic). */
+ * align_corners=False; strides = the L feature strides (HOST floats; reference-point arithmetic).  Softmax over all L*P
+ * points of a head.  P == 4 (else -2); 1 <= L <= 4, E % 32 == 0, E / H % 4 == 0, E / H <= 32, head_ld % 4 == 0,
+ * value_ld >= (H - 1) * head_ld + E / H and % 4 == 0, value and out 16-byte aligned; B * sum X*Y*Z < 2^31. */
 int occ_ms_deform_attn(const float* value, int value_ld, int head_ld, const float* ow, float* out, int L, int B,
                        const int* grids, const float* strides, int E, int H, int P, occ_stream_t stream);
 /* FPN step (:228-240): out_s (S32) = GroupNorm(cur raw lateral-conv output, stats) + trilinear upsample
- * (align_corners=False) of coarse (B, Xc, Yc, Zc, C) fp32 */
+ * (align_corners=False) of coarse (B, Xc, Yc, Zc, C) fp32, any size ratio (exact x2 on every axis takes a tiled kernel).
+ * C % 32 == 0, C <= 4096, groups divides C; cur, coarse and out_s 16-byte aligned; GroupNorm eps 1e-5. */
 int occ_gn_upsample_add(const float* cur, const double* stats, const float* gw, const float* gb, int groups,
                         const float* coarse, float* out_s, int B, int X, int Y, int Z, int Xc, int Yc, int Zc, int C,
                         occ_stream_t stream);

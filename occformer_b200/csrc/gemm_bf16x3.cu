@@ -523,8 +523,11 @@ namespace occ {
 
 // GroupNorm statistics of a finished (B, rows_per_sample, C) tensor (split-K conv outputs, the neck's input convs):
 // stats[b][g] += (sum, sumsq), C % 4 == 0, any cpg with at most MAX_STAT_GROUPS groups.
-// One CTA = 32 rows; thread t owns the float4 column t (t + blockDim.x, ...): eight independent row loads in flight, fp32
-// sums over the 32 rows, fp64 per group in shared memory, one fp64 global atomic per (CTA, group, moment).
+// One CTA = 32 rows; thread t owns the float4 column t (t + blockDim.x, ...): eight independent row loads in flight, fp64
+// sums over the 32 rows, fp64 per group in shared memory, one fp64 global atomic per (CTA, group, moment).  The sums are
+// fp64 from the first row on: the consumer takes var = sumsq / n - mean^2, which cancels ~(mean / std)^2 of the digits
+// of sumsq, and fp32 column sums lost up to 1e-5 of a group's spread at mean / std = 100 (the kernel is bound by its
+// loads).
 constexpr int GS_ROWS = 32;
 __global__ void __launch_bounds__(256)
 conv_gn_stats_kernel(const float* __restrict__ x, double* __restrict__ stats, int rows_per_sample, int C, int cpg) {
@@ -538,23 +541,23 @@ conv_gn_stats_kernel(const float* __restrict__ x, double* __restrict__ stats, in
   __syncthreads();
   const float4* base = reinterpret_cast<const float4*>(x + ((size_t)b * rows_per_sample + r0) * C);
   for (int c4 = threadIdx.x; c4 < C4; c4 += blockDim.x) {
-    float4 s = make_float4(0.f, 0.f, 0.f, 0.f), q = make_float4(0.f, 0.f, 0.f, 0.f);
+    double s[4] = {0.0, 0.0, 0.0, 0.0}, q[4] = {0.0, 0.0, 0.0, 0.0};
 #pragma unroll 8
     for (int r = 0; r < nr; ++r) {
       const float4 v = __ldg(base + (size_t)r * C4 + c4);
-      s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
-      q.x = fmaf(v.x, v.x, q.x); q.y = fmaf(v.y, v.y, q.y); q.z = fmaf(v.z, v.z, q.z); q.w = fmaf(v.w, v.w, q.w);
+      const double d[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) { s[j] += d[j]; q[j] = fma(d[j], d[j], q[j]); }
     }
     const int c = c4 << 2;
     if (cpg % 4 == 0) {  // the four columns share a group
-      atomicAdd(&sg[2 * (c / cpg)], (double)((s.x + s.y) + (s.z + s.w)));
-      atomicAdd(&sg[2 * (c / cpg) + 1], (double)((q.x + q.y) + (q.z + q.w)));
+      atomicAdd(&sg[2 * (c / cpg)], (s[0] + s[1]) + (s[2] + s[3]));
+      atomicAdd(&sg[2 * (c / cpg) + 1], (q[0] + q[1]) + (q[2] + q[3]));
     } else {
-      const float sv[4] = {s.x, s.y, s.z, s.w}, qv[4] = {q.x, q.y, q.z, q.w};
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        atomicAdd(&sg[2 * ((c + j) / cpg)], (double)sv[j]);
-        atomicAdd(&sg[2 * ((c + j) / cpg) + 1], (double)qv[j]);
+        atomicAdd(&sg[2 * ((c + j) / cpg)], s[j]);
+        atomicAdd(&sg[2 * ((c + j) / cpg) + 1], q[j]);
       }
     }
   }

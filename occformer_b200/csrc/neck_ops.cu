@@ -67,6 +67,11 @@ token_prep_kernel(const float* __restrict__ in, const float* __restrict__ ln_w, 
 #pragma unroll
   for (int c = 0; c < NCH; ++c) v[c] = __ldcs(in + row * C + c * 32 + lane);
   if (ln_w) {
+    // two-pass on the row shifted by its first element (lane 0's element 0): for a row whose offset dwarfs its spread
+    // the shifted values are exact and small, so the fp32 sums lose no digits to the offset
+    const float shift = __shfl_sync(0xffffffffu, v[0], 0);
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) v[c] -= shift;
     float s = 0.f;
 #pragma unroll
     for (int c = 0; c < NCH; ++c) s += v[c];
@@ -533,6 +538,8 @@ extern "C" int occ_gn_upsample_add(const float* cur, const double* stats, const 
   OCC_REQUIRE(cur && stats && gw && gb && coarse && out_s);
   OCC_REQUIRE(B > 0 && X > 0 && Y > 0 && Z > 0 && Xc > 0 && Yc > 0 && Zc > 0 && C % 32 == 0 && groups > 0 && C % groups == 0);
   OCC_REQUIRE(B <= 65535 && C <= 4096);
+  OCC_REQUIRE(((reinterpret_cast<uintptr_t>(cur) | reinterpret_cast<uintptr_t>(coarse) |
+                reinterpret_cast<uintptr_t>(out_s)) & 15) == 0);  // float4 loads and stores
   const long long V = (long long)X * Y * Z;
   OCC_REQUIRE(V < (1ll << 31));
   if (X == 2 * Xc && Y == 2 * Yc && Z == 2 * Zc && B <= 65535 && C / 32 <= 65535) {
