@@ -174,6 +174,16 @@ int occ_depthnet_gap_branch(const float* in, float* ws, const float* w, const fl
  * n*H*W, 9*C/groups) S32: column k*Cg + c of group g = channel g*Cg + c at point k, Cg = C/groups a multiple of 32. */
 int occ_deform_im2col(const float* x, const float* off, int off_ld, float* cols, int n, int H, int W, int C, int groups,
                       occ_stream_t stream);
+/* Modulated deformable im2col of mmcv ModulatedDeformConv2dPack (DCNv2, 3x3, stride 1, padding 1, dilation 1, one
+ * deformable group; mmcv-full 1.4.0 mmcv/ops/modulated_deform_conv.py forward, modulated_deform_conv_cuda_kernel.cuh
+ * modulated_deformable_im2col_gpu_kernel / dmcn_im2col_bilinear), the 3x3 conv2 of ResNetDCN's DCN Bottlenecks:
+ * x (n, H, W, C) S32, C % 32 == 0; off (n*H*W, off_ld) fp32, off_ld >= 27, the conv_offset output rows: column 2k / 2k+1
+ * is the (dy, dx) offset of kernel point k = ky*3 + kx, column 18 + k its mask logit (chunk(out, 3) -> o1, o2, mask;
+ * offset = cat(o1, o2); mask = sigmoid(mask), applied here); columns 27.. are not read.  Sampling as occ_deform_im2col
+ * (h = y - 1 + ky + dy, inside test h > -1 && w > -1 && h < H && w < W, corners outside the map = 0), then col = val *
+ * sigmoid(logit).  cols (n*H*W, 9*C) S32: column k*C + c = channel c at point k.  x and cols 16-byte aligned. */
+int occ_modulated_deform_im2col(const float* x, const float* off, int off_ld, float* cols, int n, int H, int W, int C,
+                                occ_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Image encoder of the nuScenes R50 model (projects/configs/occformer_nusc/occformer_nusc_r50_256x704.py:65-79):

@@ -5,7 +5,7 @@ projects/mmdet3d_plugin of the reference; all arithmetic runs in csrc/libocc_b20
 """
 from .registry import ATTENTION, BACKBONES, HEADS, NECKS, POSITIONAL_ENCODING  # noqa: F401
 from .encoder import DualpathTransformerBlock, OccupancyEncoder  # noqa: F401
-from .image_encoder import SECONDFPN, ResNet  # noqa: F401
+from .image_encoder import SECONDFPN, ResNet, ResNetDCN  # noqa: F401
 from .efficientnet import CustomEfficientNet  # noqa: F401
 from .view_transformer import ViewTransformerLiftSplatShootVoxel, bev_pool  # noqa: F401
 from .neck import MSDeformAttnPixelDecoder3D, MultiScaleDeformableAttention3D  # noqa: F401

@@ -1,6 +1,7 @@
 // The kernels of DepthNet (P/occformer/image2bev/ViewTransformerLSSBEVDepth.py:435-504) that are not convolutions: the
 // camera-aware SE gates, their application to the reduced features, and the deformable im2col of the DCN
-// (mmcv-full 1.4.0 DeformConv2dPack, DCNv1).  Every contraction of DepthNet goes through occ_conv_bf16x3 /
+// (mmcv-full 1.4.0 DeformConv2dPack, DCNv1), whose modulated instantiation serves the DCNv2 convs of the image encoder's
+// ResNetDCN (ModulatedDeformConv2dPack).  Every contraction of DepthNet goes through occ_conv_bf16x3 /
 // occ_conv_slice_bf16x3; activations are channel-last rows (image, y, x) of C floats.
 #include "occ_common.cuh"
 #include "occ_ptx.cuh"
@@ -69,6 +70,9 @@ se_apply_kernel(const float* __restrict__ x, const float* __restrict__ gates, fl
 // deformable_im2col_bilinear (3x3, stride 1, padding 1, dilation 1, one deformable group), in the same fp32 expression
 // order.  The input is read in S32 and rebuilt as hi + lo.  cols: (groups, rows, 9 * Cg) S32, column k * Cg + c of
 // group g = channel g * Cg + c at kernel point k.
+// MOD (DCNv2, mmcv's modulated_deformable_im2col_gpu_kernel / dmcn_im2col_bilinear, same sampling rules): the sample is
+// multiplied by mask = sigmoid(off[18 + k]) after the bilinear sum (col = val * mask); groups == 1.
+template <bool MOD>
 __global__ void __launch_bounds__(256)
 deform_im2col_kernel(const float* __restrict__ x, const float* __restrict__ off, int off_ld, float* __restrict__ cols,
                      long long rows, int H, int W, int C, int Cg) {
@@ -83,6 +87,8 @@ deform_im2col_kernel(const float* __restrict__ x, const float* __restrict__ off,
   const int py = pix / W, px = pix - (pix / W) * W;
   const float h = (float)(py - 1 + k / 3) + __ldg(off + p * off_ld + 2 * k);
   const float w = (float)(px - 1 + k % 3) + __ldg(off + p * off_ld + 2 * k + 1);
+  float mask = 1.f;
+  if constexpr (MOD) mask = 1.f / (1.f + expf(-__ldg(off + p * off_ld + 18 + k)));
   const bool inside = h > -1.f && w > -1.f && h < (float)H && w < (float)W;
   const int h_low = (int)floorf(h), w_low = (int)floorf(w);
   const int h_high = h_low + 1, w_high = w_low + 1;
@@ -105,6 +111,7 @@ deform_im2col_kernel(const float* __restrict__ x, const float* __restrict__ off,
     o.y = w1 * v1.y + w2 * v2.y + w3 * v3.y + w4 * v4.y;
     o.z = w1 * v1.z + w2 * v2.z + w3 * v3.z + w4 * v4.z;
     o.w = w1 * v1.w + w2 * v2.w + w3 * v3.w + w4 * v4.w;
+    if constexpr (MOD) o = make_float4(o.x * mask, o.y * mask, o.z * mask, o.w * mask);
     const int g = c0 / Cg, cl = c0 - g * Cg;
     store_split4(cols + ((size_t)g * rows + p) * (9 * Cg), k * Cg + cl, o);
   }
@@ -145,7 +152,20 @@ extern "C" int occ_deform_im2col(const float* x, const float* off, int off_ld, f
   const long long rows = (long long)n * H * W;
   const long long warps = rows * 9;
   OCC_REQUIRE((warps + 7) / 8 < (1ll << 31));
-  deform_im2col_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, stream>>>(x, off, off_ld, cols, rows, H, W, C, C / groups);
+  deform_im2col_kernel<false><<<(unsigned)((warps + 7) / 8), 256, 0, stream>>>(x, off, off_ld, cols, rows, H, W, C,
+                                                                              C / groups);
+  OCC_LAUNCH_CHECK();
+  return OCC_OK;
+}
+
+extern "C" int occ_modulated_deform_im2col(const float* x, const float* off, int off_ld, float* cols, int n, int H, int W,
+                                           int C, cudaStream_t stream) {
+  OCC_REQUIRE(x && off && cols && n > 0 && H > 0 && W > 0 && C > 0 && C % 32 == 0 && off_ld >= 27);
+  OCC_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(cols)) & 15) == 0);
+  const long long rows = (long long)n * H * W;
+  const long long warps = rows * 9;
+  OCC_REQUIRE((warps + 7) / 8 < (1ll << 31));
+  deform_im2col_kernel<true><<<(unsigned)((warps + 7) / 8), 256, 0, stream>>>(x, off, off_ld, cols, rows, H, W, C, C);
   OCC_LAUNCH_CHECK();
   return OCC_OK;
 }

@@ -101,6 +101,23 @@ class SELayer(nn.Module):
         return x * self.gate(self.conv_expand(self.act1(self.conv_reduce(x_se))))
 
 
+def deform_columns(x, off):
+    """The sampling columns of a 3x3, stride 1, padding 1 deformable conv with one deformable group (mmcv DeformConv2d /
+    ModulatedDeformConv2d): x (B, C, H, W), off (B, >= 18, H, W) whose channel 2k / 2k+1 is the (dy, dx) offset of
+    kernel point k = ky*3 + kx -> (B, C, 9, H, W), point k sampled at (y - 1 + ky + dy, x - 1 + kx + dx), bilinear with
+    zeros outside the map (``grid_sample``)."""
+    B, C, H, W = x.shape
+    ys = torch.arange(H, device=x.device, dtype=x.dtype).view(1, H, 1)
+    xs = torch.arange(W, device=x.device, dtype=x.dtype).view(1, 1, W)
+    cols = []
+    for k in range(9):
+        py = ys + (k // 3 - 1) + off[:, 2 * k]
+        px = xs + (k % 3 - 1) + off[:, 2 * k + 1]
+        grid = torch.stack((2.0 * px / max(W - 1, 1) - 1.0, 2.0 * py / max(H - 1, 1) - 1.0), dim=-1)
+        cols.append(F.grid_sample(x, grid, mode="bilinear", padding_mode="zeros", align_corners=True))
+    return torch.stack(cols, dim=2)
+
+
 class DCN(nn.Module):
     """mmcv ``DeformConv2dPack`` (DCNv1): 3x3, stride 1, padding 1, ``groups`` weight groups, one deformable group.
     Parameters: ``weight`` (out, in/groups, 3, 3) without bias and ``conv_offset`` = Conv2d(in, 18, 3, padding 1) whose
@@ -119,16 +136,7 @@ class DCN(nn.Module):
 
     def forward(self, x):
         B, C, H, W = x.shape
-        off = self.conv_offset(x)
-        ys = torch.arange(H, device=x.device, dtype=x.dtype).view(1, H, 1)
-        xs = torch.arange(W, device=x.device, dtype=x.dtype).view(1, 1, W)
-        cols = []
-        for k in range(9):
-            py = ys + (k // 3 - 1) + off[:, 2 * k]
-            px = xs + (k % 3 - 1) + off[:, 2 * k + 1]
-            grid = torch.stack((2.0 * px / max(W - 1, 1) - 1.0, 2.0 * py / max(H - 1, 1) - 1.0), dim=-1)
-            cols.append(F.grid_sample(x, grid, mode="bilinear", padding_mode="zeros", align_corners=True))
-        col = torch.stack(cols, dim=2)  # (B, C, 9, H, W)
+        col = deform_columns(x, self.conv_offset(x))  # (B, C, 9, H, W)
         g = self.groups
         col = col.view(B, g, C // g, 9, H, W)
         w = self.weight.view(g, -1, C // g, 9)  # (g, out/g, in/g, 9)

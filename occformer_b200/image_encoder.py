@@ -1,9 +1,12 @@
-"""Image encoder of the nuScenes R50 model: the stage in front of DepthNet that turns camera images into feature maps.
+"""Image encoder of the nuScenes R50 and R101 models: the stage in front of DepthNet that turns camera images into
+feature maps.
 
     ResNet / Bottleneck      mmdet 2.14.0 mmdet/models/backbones/resnet.py (depth 50, style 'pytorch')
+    ResNetDCN                the same ResNet at depth 50 / 101, style 'pytorch' / 'caffe', with DCNv2 3x3 convs
+    ModulatedDeformConv2dPack  mmcv-full 1.4.0 mmcv/ops/modulated_deform_conv.py (the 'DCNv2' conv layer)
     SECONDFPN                mmdetection3d/mmdet3d/models/necks/second_fpn.py:11-91
     config                   projects/configs/occformer_nusc/occformer_nusc_r50_256x704.py:65-79 (img_backbone,
-                             img_neck; the panoptic config uses the same two)
+                             img_neck; the panoptic config uses the same two), occformer_nusc_r101_896x1600.py:67-84
 
 Both modules take the reference's constructor kwargs and have its exact ``state_dict`` keys (ResNet's are torchvision's
 ``resnet50`` keys without ``fc.*``), so a reference checkpoint's ``img_backbone.*`` / ``img_neck.*`` entries load with
@@ -21,8 +24,8 @@ level is unmodified (common.twin_of), else it splits the level itself; its own o
 a ``channels_last`` map, which survives the reference glue's ``.view`` calls and which DepthNet splits without a
 transpose.
 
-``ResNet`` and ``SECONDFPN`` are general mmdet / mmdet3d names: they are registered in this package's local registries
-only, never forced into the upstream ones (INTEGRATION.md shows the opt-in).
+``ResNet``, ``ResNetDCN`` and ``SECONDFPN`` are registered in this package's local registries only, never forced into
+the upstream ones (INTEGRATION.md shows the opt-in).
 """
 import torch
 import torch.nn as nn
@@ -30,25 +33,64 @@ import torch.nn.functional as F
 
 from . import ops
 from .common import PreparedModule, attach_twin, batchnorm, fold_bn, round32, twin_of
+from .depthnet import deform_columns
 from .registry import BACKBONES, NECKS
+
+# ---------------------------------------------------------------------------------------------------------- DCNv2
+class ModulatedDeformConv2dPack(nn.Module):
+    """mmcv-full 1.4.0 ``ModulatedDeformConv2dPack`` (mmcv/ops/modulated_deform_conv.py; the 'DCNv2' conv layer of mmdet's
+    Bottleneck, built with bias=False): 3x3, stride 1, padding 1, dilation 1, groups 1, one deformable group.
+    Parameters ``weight`` (out, in, 3, 3) and ``conv_offset`` = Conv2d(in, 27, 3, padding 1, bias).  Forward, as mmcv's:
+    ``o1, o2, mask = chunk(conv_offset(x), 3, dim=1)``, ``offset = cat(o1, o2)``, ``mask = sigmoid(mask)``; kernel point
+    k = ky*3 + kx takes (dy, dx) from offset channels 2k / 2k+1 and samples x at h = (y - 1 + ky) + dy, w = (x - 1 + kx) +
+    dx, bilinear, zero unless h > -1 && w > -1 && h < H && w < W and each corner outside the map zero
+    (modulated_deform_conv_cuda_kernel.cuh modulated_deformable_im2col_gpu_kernel / dmcn_im2col_bilinear); the column is
+    val * mask_k, then the contraction with ``weight``.  Here the sampling is depthnet.deform_columns (``grid_sample``
+    with zero padding, which zeroes every sample with h <= -1 or h >= H as mmcv's inside test does)."""
+
+    def __init__(self, in_channels, out_channels, kernel_size=3, stride=1, padding=1, dilation=1, groups=1,
+                 deform_groups=1, bias=False):
+        super().__init__()
+        if kernel_size not in (3, (3, 3)) or (stride, padding, dilation, groups, deform_groups) != (1,) * 5 or bias:
+            raise NotImplementedError("occformer_b200.ModulatedDeformConv2dPack: 3x3, stride 1, padding 1, dilation 1, "
+                                      "groups 1, deform_groups 1, bias=False only")
+        self.in_channels, self.out_channels = in_channels, out_channels
+        self.weight = nn.Parameter(torch.empty(out_channels, in_channels, 3, 3))
+        nn.init.kaiming_uniform_(self.weight, nonlinearity="relu")
+        self.conv_offset = nn.Conv2d(in_channels, 27, 3, stride=1, padding=1, bias=True)
+        nn.init.zeros_(self.conv_offset.weight)
+        nn.init.zeros_(self.conv_offset.bias)
+
+    def forward(self, x):
+        C = x.shape[1]
+        o1, o2, mask = torch.chunk(self.conv_offset(x), 3, dim=1)
+        col = deform_columns(x, torch.cat((o1, o2), dim=1)) * torch.sigmoid(mask).unsqueeze(1)  # (B, C, 9, H, W)
+        return torch.einsum("bckhw,ock->bohw", col, self.weight.view(self.out_channels, C, 9))
+
 
 # ---------------------------------------------------------------------------------------------------------- ResNet
 class Bottleneck(nn.Module):
-    """mmdet Bottleneck, style 'pytorch' (the stride is on the 3x3 conv): relu(bn3(conv3(relu(bn2(conv2(relu(bn1(
-    conv1(x)))))))) + identity), identity = downsample(x) when present."""
+    """mmdet Bottleneck: relu(bn3(conv3(relu(bn2(conv2(relu(bn1(conv1(x)))))))) + identity), identity = downsample(x) when
+    present.  Style 'pytorch' puts the stride on the 3x3 conv2, style 'caffe' on the 1x1 conv1; dcn: conv2 is a
+    ModulatedDeformConv2dPack (stride 1 only)."""
     expansion = 4
 
-    def __init__(self, inplanes, planes, stride=1, downsample=None, norm_cfg=None):
+    def __init__(self, inplanes, planes, stride=1, downsample=None, norm_cfg=None, style="pytorch", dcn=False):
         super().__init__()
-        self.conv1 = nn.Conv2d(inplanes, planes, 1, bias=False)
+        s1, s2 = (stride, 1) if style == "caffe" else (1, stride)
+        self.conv1 = nn.Conv2d(inplanes, planes, 1, stride=s1, bias=False)
         self.bn1 = batchnorm(norm_cfg, planes, 1e-5)
-        self.conv2 = nn.Conv2d(planes, planes, 3, stride=stride, padding=1, bias=False)
+        if dcn:
+            assert s2 == 1
+            self.conv2 = ModulatedDeformConv2dPack(planes, planes, 3, padding=1)
+        else:
+            self.conv2 = nn.Conv2d(planes, planes, 3, stride=s2, padding=1, bias=False)
         self.bn2 = batchnorm(norm_cfg, planes, 1e-5)
         self.conv3 = nn.Conv2d(planes, planes * self.expansion, 1, bias=False)
         self.bn3 = batchnorm(norm_cfg, planes * self.expansion, 1e-5)
         self.relu = nn.ReLU(inplace=True)
         self.downsample = downsample
-        self.stride = stride
+        self.stride, self.style, self.dcn = stride, style, dcn
 
     def forward(self, x):
         out = self.relu(self.bn1(self.conv1(x)))
@@ -68,6 +110,8 @@ class ResNet(PreparedModule):
     touch the file system; load a checkpoint with load_state_dict.  Options this implementation does not have raise
     NotImplementedError naming the kwarg."""
     arch_settings = {50: (3, 4, 6, 3)}
+    styles = ("pytorch",)
+    scope = "depth 50, style 'pytorch', BatchNorm, strides (1, 2, 2, 2), dilation 1, plain stem"
 
     def __init__(self, depth, in_channels=3, stem_channels=None, base_channels=64, num_stages=4, strides=(1, 2, 2, 2),
                  dilations=(1, 1, 1, 1), out_indices=(0, 1, 2, 3), style="pytorch", deep_stem=False, avg_down=False,
@@ -77,21 +121,18 @@ class ResNet(PreparedModule):
         super().__init__()
 
         def unsupported(kwarg, value):
-            raise NotImplementedError(f"occformer_b200.ResNet: {kwarg}={value!r} is not supported (depth 50, "
-                                      "style 'pytorch', BatchNorm, strides (1, 2, 2, 2), dilation 1, plain stem)")
+            raise NotImplementedError(f"occformer_b200.{type(self).__name__}: {kwarg}={value!r} is not supported "
+                                      f"({self.scope})")
 
         if depth not in self.arch_settings:
             unsupported("depth", depth)
-        if style != "pytorch":
+        if style not in self.styles:
             unsupported("style", style)
         if deep_stem:
             unsupported("deep_stem", deep_stem)
         if avg_down:
             unsupported("avg_down", avg_down)
-        if dcn is not None:
-            unsupported("dcn", dcn)
-        if any(stage_with_dcn):
-            unsupported("stage_with_dcn", stage_with_dcn)
+        self.stage_dcn = self._dcn_stages(dcn, stage_with_dcn, style, strides, num_stages, unsupported)
         if plugins:
             unsupported("plugins", plugins)
         if in_channels != 3:
@@ -106,7 +147,7 @@ class ResNet(PreparedModule):
             unsupported("conv_cfg", conv_cfg)
         if any(not 0 <= i < num_stages for i in out_indices):
             unsupported("out_indices", out_indices)
-        self.depth, self.num_stages, self.out_indices = depth, num_stages, tuple(out_indices)
+        self.depth, self.num_stages, self.out_indices, self.style = depth, num_stages, tuple(out_indices), style
         self.base_channels = base_channels
         self.stem_channels = stem_channels or base_channels
         self.conv1 = nn.Conv2d(3, self.stem_channels, 7, stride=2, padding=3, bias=False)
@@ -121,11 +162,21 @@ class ResNet(PreparedModule):
             if stride != 1 or inplanes != planes * Bottleneck.expansion:
                 downsample = nn.Sequential(nn.Conv2d(inplanes, planes * Bottleneck.expansion, 1, stride=stride, bias=False),
                                            batchnorm(norm_cfg, planes * Bottleneck.expansion, 1e-5))
-            layer = [Bottleneck(inplanes, planes, stride, downsample, norm_cfg)]
+            kw = dict(norm_cfg=norm_cfg, style=style, dcn=self.stage_dcn[i])
+            layer = [Bottleneck(inplanes, planes, stride, downsample, **kw)]
             inplanes = planes * Bottleneck.expansion
-            layer += [Bottleneck(inplanes, planes, 1, None, norm_cfg) for _ in range(1, blocks)]
+            layer += [Bottleneck(inplanes, planes, 1, None, **kw) for _ in range(1, blocks)]
             self.add_module(f"layer{i + 1}", nn.Sequential(*layer))
             self.res_layers.append(f"layer{i + 1}")
+
+    @staticmethod
+    def _dcn_stages(dcn, stage_with_dcn, style, strides, num_stages, unsupported):
+        """-> per stage whether its 3x3 convs are DCNv2; ResNet has none"""
+        if dcn is not None:
+            unsupported("dcn", dcn)
+        if any(stage_with_dcn):
+            unsupported("stage_with_dcn", stage_with_dcn)
+        return (False,) * num_stages
 
     def forward(self, x):
         if x.is_cuda:
@@ -138,14 +189,14 @@ class ResNet(PreparedModule):
         """Eval BatchNorms folded into the convs before them (natural layouts, fp32 on the parameters' device):
         {"stem": (w (C0, 3, 7, 7), b), "blocks": [(stride, (w1, b1), (w2, b2), (w3, b3), (wd, bd) | None), ...]} with the
         blocks of all stages in order."""
-        F_ = {"stem": fold_bn(self.conv1.weight, None, self.bn1), "blocks": []}
-        for name in self.res_layers:
-            for blk in getattr(self, name):
-                ds = blk.downsample
-                F_["blocks"].append((blk.stride, fold_bn(blk.conv1.weight, None, blk.bn1),
-                                     fold_bn(blk.conv2.weight, None, blk.bn2), fold_bn(blk.conv3.weight, None, blk.bn3),
-                                     None if ds is None else fold_bn(ds[0].weight, None, ds[1])))
-        return F_
+        return {"stem": fold_bn(self.conv1.weight, None, self.bn1),
+                "blocks": [self._fold_block(blk) for name in self.res_layers for blk in getattr(self, name)]}
+
+    @staticmethod
+    def _fold_block(blk):
+        ds = blk.downsample
+        return (blk.stride, fold_bn(blk.conv1.weight, None, blk.bn1), fold_bn(blk.conv2.weight, None, blk.bn2),
+                fold_bn(blk.conv3.weight, None, blk.bn3), None if ds is None else fold_bn(ds[0].weight, None, ds[1]))
 
     @torch.no_grad()
     def _prepare(self):
@@ -155,9 +206,16 @@ class ResNet(PreparedModule):
         w, b = F_["stem"]
         wm = w.permute(0, 2, 3, 1).reshape(w.shape[0], 147)
         wm = torch.cat([wm, wm.new_zeros(w.shape[0], ops.STEM_COLS - 147)], dim=1)
-        rp = lambda wb: None if wb is None else (ops.repack_conv_weight(wb[0])[0], wb[1])  # noqa: E731
-        return {"stem": (ops.split_weight(wm), b),
-                "blocks": [(s, rp(c1), rp(c2), rp(c3), rp(d)) for s, c1, c2, c3, d in F_["blocks"]]}
+        return {"stem": (ops.split_weight(wm), b), "blocks": [self._prepare_block(fb) for fb in F_["blocks"]]}
+
+    @staticmethod
+    def _repack(wb):
+        return None if wb is None else (ops.repack_conv_weight(wb[0])[0], wb[1])
+
+    @classmethod
+    def _prepare_block(cls, fb):
+        s, c1, c2, c3, d = fb
+        return (s, cls._repack(c1), cls._repack(c2), cls._repack(c3), cls._repack(d))
 
     def _check_cuda_contract(self, x):
         need = []
@@ -172,7 +230,8 @@ class ResNet(PreparedModule):
         if self.training:
             need.append("eval mode (the CUDA forward applies the BatchNorms' running statistics; call .eval())")
         if need:
-            raise RuntimeError(f"occformer_b200: ResNet's CUDA forward needs {'; '.join(need)} -- got x {tuple(x.shape)}, "
+            raise RuntimeError(f"occformer_b200: {type(self).__name__}'s CUDA forward needs {'; '.join(need)} -- got x "
+                               f"{tuple(x.shape)}, "
                                f"stem_channels {self.stem_channels}, base_channels {self.base_channels}")
 
     @torch.no_grad()
@@ -215,6 +274,73 @@ class ResNet(PreparedModule):
             if i in self.out_indices:
                 outs.append(x)
         return tuple(outs)
+
+
+@BACKBONES.register_module(upstream=False)
+class ResNetDCN(ResNet):
+    """mmdet 2.14.0 ``ResNet`` with the options of the nuScenes R101 config (occformer_nusc_r101_896x1600.py:68-79): depth
+    50 or 101, style 'pytorch' or 'caffe' (mmdet's Bottleneck puts the stage stride on conv1 in caffe style), and
+    ``dcn=dict(type='DCNv2', deform_groups=1, fallback_on_stride=False)`` on the stages of ``stage_with_dcn``, whose 3x3
+    conv2 is then a ModulatedDeformConv2dPack.  A DCN on a strided conv2 (style 'pytorch', stages 2-4) is not supported;
+    everything else is ResNet's: same keys (plus ``layer{i}.{j}.conv2.conv_offset.{weight,bias}``), same kwargs, the
+    same NotImplementedError for the options neither has.  ``norm_cfg`` type 'BN2d' is BatchNorm.
+
+    CUDA forward of a DCN Bottleneck: conv1 (1x1, stride s in caffe style, S32 out) -> conv_offset (3x3 conv, Cout
+    padded 27 -> 32, fp32 rows) -> ops.modulated_deform_im2col -> GEMM of the columns with the tap-major conv2 weight (bn2
+    folded, ReLU, S32 out) -> conv3 + identity + ReLU -> split: two launches more than a plain Bottleneck."""
+    arch_settings = {50: (3, 4, 6, 3), 101: (3, 4, 23, 3)}
+    styles = ("pytorch", "caffe")
+    scope = ("depth 50 or 101, style 'pytorch' or 'caffe', dcn DCNv2 with deform_groups 1 and fallback_on_stride "
+             "False on stride-1 3x3 convs only (a DCN in stages 2-4 needs style 'caffe'), BatchNorm, strides (1, 2, 2, 2), "
+             "dilation 1, plain stem")
+
+    @staticmethod
+    def _dcn_stages(dcn, stage_with_dcn, style, strides, num_stages, unsupported):
+        if dcn is None:  # mmdet: stage_with_dcn only matters with a dcn
+            return (False,) * num_stages
+        d = dict(dcn)
+        if d.get("type") != "DCNv2" or d.get("deform_groups", 1) != 1 or d.get("fallback_on_stride", False) or \
+                set(d) - {"type", "deform_groups", "fallback_on_stride"}:
+            unsupported("dcn", dcn)
+        if len(stage_with_dcn) != num_stages:
+            unsupported("stage_with_dcn", stage_with_dcn)
+        if style != "caffe" and any(w and s != 1 for w, s in zip(stage_with_dcn, strides)):
+            unsupported("stage_with_dcn", stage_with_dcn)
+        return tuple(bool(w) for w in stage_with_dcn)
+
+    @staticmethod
+    def _fold_block(blk):
+        """ResNet's block entry + (caffe, conv_offset (w (32, C, 3, 3), b (32)) zero-padded from 27 channels | None)"""
+        off = None
+        if blk.dcn:
+            co = blk.conv2.conv_offset
+            w, b = co.weight.detach().float(), co.bias.detach().float()
+            off = (torch.cat([w, w.new_zeros(32 - w.shape[0], *w.shape[1:])]).contiguous(),
+                   torch.cat([b, b.new_zeros(32 - b.shape[0])]).contiguous())
+        return ResNet._fold_block(blk) + (blk.style == "caffe", off)
+
+    @classmethod
+    def _prepare_block(cls, fb):
+        return super()._prepare_block(fb[:5]) + (fb[5], cls._repack(fb[6]))
+
+    @staticmethod
+    def _bottleneck_cuda(p, x, x_s):
+        """ResNet._bottleneck_cuda for an entry of ResNetDCN._prepare()["blocks"]: stride on conv1 when caffe, conv2 a
+        DCNv2 when the entry has conv_offset weights."""
+        s, (w1, b1), (w2, b2), (w3, b3), ds, caffe, off = p
+        s1, s2 = (s, 1) if caffe else (1, s)
+        k1, k3 = (1, 1, 1), (3, 3, 1)
+        t = ops.conv(x_s, w1, k1, stride=s1, bias=b1, act=1, split_out=True)
+        if off is None:
+            t = ops.conv(t, w2, k3, stride=s2, bias=b2, act=1, split_out=True)
+        else:
+            n, h, w, _, C = t.shape
+            o = ops.conv(t, off[0], k3, bias=off[1]).view(n * h * w, 32)
+            cols = ops.modulated_deform_im2col(t, o, n, h, w)
+            t = ops.gemm(cols, w2, bias=b2, act=1, split_out=True).view(n, h, w, 1, C)
+        ident = x if ds is None else ops.conv(x_s, ds[0], k1, stride=s, bias=ds[1])
+        out = ops.conv(t, w3, k1, bias=b3, residual=ident, act=1)
+        return out, ops.to_split(out)
 
 
 # ---------------------------------------------------------------------------------------------------------- SECONDFPN

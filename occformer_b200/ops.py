@@ -395,6 +395,17 @@ def deform_im2col(x_s, off, n, H, W, groups):
     return cols
 
 
+def modulated_deform_im2col(x_s, off, n, H, W):
+    """DCNv2 sampling columns: x_s (n*H*W, C) S32, off (n*H*W, >= 27) fp32 conv_offset rows (dy, dx of point k in columns
+    2k, 2k+1, its mask logit in column 18 + k) -> (n*H*W, 9*C) S32, column k*C + c = sigmoid(logit_k) * sample."""
+    C = x_s.shape[-1]
+    rows = n * H * W
+    assert x_s.numel() == rows * C and off.dim() == 2 and off.shape[0] == rows
+    cols = torch.empty((rows, 9 * C), dtype=torch.float32, device=x_s.device)
+    _call("occ_modulated_deform_im2col", x_s, off, off.shape[1], cols, n, H, W, C)
+    return cols
+
+
 # ----------------------------------------------------------------------------------------------- image encoder
 STEM_COLS = 160  # the 147 (ky, kx, c) columns of the 7x7x3 stem, padded to whole S32 chunks
 

@@ -373,6 +373,32 @@ def make_resnet_state(seed=0, calib_shape=(4, 3, 64, 96), **resnet_kwargs):
     return _calibrate_batchnorms(net, [_randn(g, *calib_shape).double()], g)
 
 
+def make_resnet_dcn_state(seed=0, depth=101, calib_shape=(1, 3, 224, 416), bn3_gain=0.05, **resnet_kwargs):
+    """state_dict of image_encoder.ResNetDCN(depth, **resnet_kwargs), made as make_resnet_state makes ResNet's (He convs,
+    bn3 weight bn3_gain * (1 + 0.1 N), BatchNorm statistics calibrated on a seeded fp64 forward of N(0,1) images of
+    calib_shape), with each DCNv2's weight He-initialised and its conv_offset He-initialised with zero bias: on the
+    calibrated, ReLU'd input of the DCN, offsets of about 1 px (std 1.07 at the R101 config; fractional positions
+    everywhere, about 3 % of the samples off the map) and mask logits of about N(0, 1) (std 1.07).
+
+    bn3_gain is smaller than make_resnet_state's 0.25 because R101 stacks 23 blocks in layer3, and a DCN block also
+    passes its input on through the sampling positions.  Measured in fp64 on the host at the R101 config (style 'caffe',
+    DCN in layer3 / layer4) as the growth of a relative perturbation of 1e-5 of every conv / DCN / BatchNorm weight,
+    layer1 .. layer4 on (1, 3, 448, 800) images: 4.1e-5, 5.0e-5, 9.2e-5, 1.8e-4 at bn3_gain 0.05; 1.1e-3 / 1.7e-3 at
+    layer3 / layer4 with 0.1 and 0.18 / 0.43 with 0.25 (chaotic: no two fp32 implementations could meet the 1e-3 gate).
+    Without the DCNs, caffe-style R101 at 0.25 reaches 7.1e-4 at layer4 ((1, 3, 224, 416) images)."""
+    from .image_encoder import ModulatedDeformConv2dPack, ResNetDCN
+    g = torch.Generator().manual_seed(seed)
+    net = _he_state(ResNetDCN(depth=depth, **resnet_kwargs), g)
+    with torch.no_grad():
+        for name, m in net.named_modules():
+            if name.endswith(".bn3"):
+                m.weight.mul_(bn3_gain)
+            elif isinstance(m, ModulatedDeformConv2dPack):
+                m.weight.copy_(_randn(g, *m.weight.shape, std=(2.0 / m.weight[0].numel()) ** 0.5))
+                m.conv_offset.bias.zero_()
+    return _calibrate_batchnorms(net, [_randn(g, *calib_shape).double()], g)
+
+
 def make_secondfpn_state(in_channels, out_channels, upsample_strides, seed=0, out_hw=(4, 8), n=2, **fpn_kwargs):
     """state_dict of image_encoder.SECONDFPN(in_channels, out_channels, upsample_strides, **fpn_kwargs) (the reference's
     deblocks.{i}.{0,1}.* keys): He-initialised (de)convs, BatchNorm affine 1 + 0.1 N / 0.1 N, running statistics
