@@ -315,6 +315,17 @@ int occ_swin_qkv_attention(const float* tokn, const float* wqkv, const float* bq
  * biased variance. */
 int occ_neck_token_prep(const float* in, const float* ln_w, const float* ln_b, const float* pos, float* out_f32,
                         float* out_s32, float* out_pos, int L, int B, const int* grids, int C, occ_stream_t stream);
+/* One encoder layer after the deformable gather, in one tensor-core kernel (csrc/neck_tail_fused.cu):
+ * y = x + att Wo^T + bo (output_proj + identity), x1 = LayerNorm(y; ln1), y2 = x1 + W2 ReLU(W1 x1 + b1) + b2 (FFN + identity),
+ * out = LayerNorm(y2; ln2) written as out_f32 (fp32), out_s32 (S32) and out_pos = out + pos[token] (S32), each optional as
+ * in occ_neck_token_prep (not all three; out_pos needs pos).  att (rows, E) S32, x (rows, E) fp32, rows = B * sum X*Y*Z
+ * of the L level grids (HOST ints); wo (E, E), w1 (F, E), w2 (E, F) S32, (out, in) row-major as in nn.Linear.
+ * E in {96, 192} (else -2, nothing enqueued), F % 32 == 0, F <= 4096; every matrix 16-byte aligned.  LayerNorm eps 1e-5,
+ * biased variance. */
+int occ_neck_layer_tail(const float* att, const float* x, const float* wo, const float* bo, const float* ln1_w,
+                        const float* ln1_b, const float* w1, const float* b1, const float* w2, const float* b2,
+                        const float* ln2_w, const float* ln2_b, const float* pos, float* out_f32, float* out_s32,
+                        float* out_pos, int L, int B, const int* grids, int E, int F, occ_stream_t stream);
 /* multi_scale_deformable_attn_pytorch + the sampling-location arithmetic of MultiScaleDeformableAttention3D.forward:
  * value (rows, value_ld) = value_proj output, head h at columns [h*head_ld, h*head_ld + E/H) (head_ld = E/H, or E/H
  * rounded up to 32 floats so that a head slice is one 128-byte line); ow (rows, H*L*P*4) = [sampling_offsets (h,l,p,(z,y,x)) | attention logits (h,l,p)];

@@ -9,9 +9,10 @@ Same constructor kwargs (cfg section ``img_bev_encoder_neck`` of occformer_nusc_
 ``state_dict`` keys.  SURVEY.md 8(f)1: the caller between the two starred subsystems -- with it the forward is connected
 (encoder pyramid -> neck -> head).
 
-All arithmetic runs in libocc_b200.so: the 1x1x1 / 3x3x3 convolutions and the six Linears of every encoder layer on the
-wgmma GEMM (split-bf16 operands, three passes, fp32-faithful), the deformable gather / LayerNorm / FPN up-sampling in
-csrc/neck_ops.cu.  Tokens are kept level-major (csrc/neck_ops.cu) so that no concatenation, split or transpose of the
+All arithmetic runs in libocc_b200.so: the 1x1x1 / 3x3x3 convolutions and the value / offset projections of every
+encoder layer on the wgmma GEMM (split-bf16 operands, three passes, fp32-faithful), the deformable gather / token
+preparation / FPN up-sampling in csrc/neck_ops.cu, and the rest of every encoder layer (output projection, both
+LayerNorms, FFN; E = 96 or 192) as one kernel in csrc/neck_tail_fused.cu.  Tokens are kept level-major (csrc/neck_ops.cu) so that no concatenation, split or transpose of the
 reference's forward exists here; tensors that feed a contraction travel in the S32 split format and carry over from the
 encoder / to the head as S32 twins (common.attach_twin).  Inference only.
 """
@@ -185,12 +186,11 @@ class MSDeformAttnPixelDecoder3D(PreparedModule):
             v = ops.gemm(x_s, W["wv"], bias=W["bv"])
             ow = ops.gemm(xq_s, W["wow"], bias=W["bow"])
             att = ops.ms_deform_attn(v, ow, grids, strides, B, E, H, self.num_points)
-            y = ops.gemm(att, W["wo"], bias=a.output_proj.bias, residual=x)
-            x1, x1_s, _ = ops.neck_token_prep(y, grids, B, ln=(lyr.norms[0].weight, lyr.norms[0].bias))
-            h = ops.gemm(x1_s, W["w1"], bias=ffn[0][0].bias, act=1, split_out=True)
-            y2 = ops.gemm(h, W["w2"], bias=ffn[1].bias, residual=x1)
+            # output_proj + residual, norms[0], FFN + residual, norms[1]: one kernel, nothing in between crosses HBM
             last = li == nl - 1
-            x, x_s, xq_s = ops.neck_token_prep(y2, grids, B, ln=(lyr.norms[1].weight, lyr.norms[1].bias), pos=pos,
+            x, x_s, xq_s = ops.neck_layer_tail(att, x, W["wo"], a.output_proj.bias, (lyr.norms[0].weight, lyr.norms[0].bias),
+                                               W["w1"], ffn[0][0].bias, W["w2"], ffn[1].bias,
+                                               (lyr.norms[1].weight, lyr.norms[1].bias), grids, B, pos=pos,
                                                want_s32=not last, want_pos=not last)
         # ---- the encoder output of every level is a contiguous channel-last tensor (:217-226)
         outs = [x[B * starts[i]:B * (starts[i] + ns[i])].view(B, *grids[i], E) for i in range(L)]

@@ -829,6 +829,25 @@ def neck_token_prep(x, grids, B, ln=None, pos=None, want_f32=True, want_s32=True
     return f32, s32, ps
 
 
+def neck_layer_tail(att, x, wo, bo, ln1, w1, b1, w2, b2, ln2, grids, B, pos=None, want_f32=True, want_s32=True,
+                    want_pos=False):
+    """One pixel-decoder encoder layer after the deformable gather, one kernel: y = x + att wo^T + bo, x1 = LN1(y),
+    out = LN2(x1 + w2 ReLU(w1 x1 + b1) + b2) -> (out fp32 | None, out S32 | None, (out + pos) S32 | None), the outputs of
+    neck_token_prep.  att (rows, E) and the weights ((out, in) as in nn.Linear) in S32; ln1 / ln2 = (weight, bias)."""
+    rows, E = x.shape
+    F = w1.shape[0]
+    assert att.shape == (rows, E) and wo.shape == (E, E) and w1.shape == (F, E) and w2.shape == (E, F)
+    assert bo.shape == (E,) and b1.shape == (F,) and b2.shape == (E,)
+    assert all(t.shape == (E,) for t in (*ln1, *ln2))
+    assert rows == B * sum(gx * gy * gz for gx, gy, gz in grids) and (pos is not None or not want_pos)
+    f32 = torch.empty_like(x) if want_f32 else None
+    s32 = torch.empty_like(x) if want_s32 else None
+    ps = torch.empty_like(x) if want_pos else None
+    _call("occ_neck_layer_tail", att, x, wo, bo, ln1[0], ln1[1], w1, b1, w2, b2, ln2[0], ln2[1],
+          pos if want_pos else None, f32, s32, ps, len(grids), B, _grids_arr(grids), E, F)
+    return f32, s32, ps
+
+
 def ms_deform_attn(value, ow, grids, strides, B, E, H, P):
     """3-D multi-scale deformable attention core on level-major rows -> (rows, E) in S32.  value (rows, H * head_ld): head h
     in columns [h*head_ld, h*head_ld + E/H) -- head_ld = E/H, or E/H rounded up to 32 (``pad_head_rows``)."""
