@@ -11,7 +11,8 @@ in place and the unchanged configs build the H100 versions).  When they are not 
 minimal local registry with the same ``register_module`` / ``build`` surface is used.
 
 The image encoder's ``ResNet`` and ``SECONDFPN`` are the exception: general mmdet / mmdet3d names, registered in the
-local registries only (``upstream=False``); INTEGRATION.md shows the opt-in.
+local registries only (``upstream=False``).  The ``OccupancyFormer`` detector resolves those names to this package's
+classes for the submodules it builds; a config built outside it opts in as INTEGRATION.md shows.
 """
 
 
@@ -86,6 +87,7 @@ class _Mirror:
 
 NECKS = _Mirror("neck", [("mmdet3d.models.builder", "NECKS"), ("mmdet.models.builder", "NECKS")])
 BACKBONES = _Mirror("backbone", [("mmdet3d.models.builder", "BACKBONES"), ("mmdet.models.builder", "BACKBONES")])
+DETECTORS = _Mirror("detector", [("mmdet.models.builder", "DETECTORS"), ("mmdet3d.models.builder", "DETECTORS")])
 HEADS = _Mirror("head", [("mmdet.models.builder", "HEADS"), ("mmdet3d.models.builder", "HEADS")])
 # mmcv 1.4.0 keeps these two in mmcv.cnn.bricks.registry (re-exported by mmcv.cnn.bricks.transformer); the reference
 # registers SinePositionalEncoding3D / MultiScaleDeformableAttention3D there

@@ -437,3 +437,54 @@ def make_efficientnet_state(arch="b7", seed=0, calib_shape=(1, 3, 384, 1280), li
             if name.endswith("linear_conv.bn"):
                 m.weight.mul_(linear_bn_gain)
     return _calibrate_batchnorms(net, [_randn(g, *calib_shape).double()], g, floor=floor)
+
+
+def make_detector_state(cfg, seed=0, cams=None):
+    """state_dict of detector.OccupancyFormer(**cfg) for a reference config's ``model`` dict, keys prefixed and in the
+    order a reference checkpoint lists them: each submodule's synthetic state above, seeded from seed .. seed + 6, plus
+    the view transformer's geometry parameters (dx, bx, nx, frustum) as the module computes them.  With ``cams`` (a
+    camera dict as workload_cameras makes) DepthNet's mlp_input BatchNorm1d gets the statistics of those cameras' MLP
+    input (variance + 1), as a trained model's would; otherwise make_depthnet_state's."""
+    from .detector import OccupancyFormer
+    from .image_encoder import ResNet, ResNetDCN
+    cfg = {k: v for k, v in cfg.items() if k != "type"}
+    det = OccupancyFormer(**cfg)
+    subs = {}
+    h = det.pts_bbox_head
+    subs["pts_bbox_head"] = make_head_state(h.decoder_embed_dims, h.num_queries, h.num_classes,
+                                            h.num_transformer_decoder_layers, h.num_transformer_feat_level,
+                                            ffn=h.ffn_channels, seed=seed)
+    bb = {k: v for k, v in cfg["img_backbone"].items() if k not in ("type", "pretrained", "init_cfg")}
+    if isinstance(det.img_backbone, ResNetDCN):
+        subs["img_backbone"] = make_resnet_dcn_state(seed + 1, **bb)
+    elif isinstance(det.img_backbone, ResNet):
+        bb.pop("depth")
+        subs["img_backbone"] = make_resnet_state(seed + 1, **bb)
+    else:
+        subs["img_backbone"] = make_efficientnet_state(seed=seed + 1, **bb)
+    neck = {k: v for k, v in cfg["img_neck"].items() if k != "type"}
+    # calibrated on the level sizes the image-encoder tests use (KITTI: stride-32 levels of 192 x 640 images)
+    subs["img_neck"] = make_secondfpn_state(seed=seed + 2, **neck, **({} if isinstance(det.img_backbone, ResNet)
+                                                                     else dict(out_hw=(6, 20))))
+    vt = det.img_view_transformer
+    dn = vt.depth_net
+    sd = make_depthnet_state(dn.in_channels, dn.mid_channels, dn.context_channels, dn.depth_channels, dn.cam_channels,
+                             seed=seed + 3)
+    if cams is not None:
+        mlp = vt.get_mlp_input(cams["rots"], cams["trans"], cams["intrins"], cams["post_rots"], cams["post_trans"],
+                               cams["bda"]).reshape(-1, dn.cam_channels)
+        sd["bn.running_mean"] = mlp.mean(0)
+        sd["bn.running_var"] = mlp.var(0, unbiased=False) + 1.0
+    vsd = {k: v for k, v in vt.state_dict().items() if not k.startswith("depth_net.")}
+    vsd.update({"depth_net." + k: v for k, v in sd.items()})
+    subs["img_view_transformer"] = vsd
+    e = cfg["img_bev_encoder_backbone"]
+    subs["img_bev_encoder_backbone"] = make_encoder_state(e["in_channels"], e["block_inplanes"], e["block_numbers"],
+                                                          e["block_strides"], seed=seed + 5)
+    n = det.img_bev_encoder_neck
+    ffn = n.state_dict()["encoder.layers.0.ffns.0.layers.0.0.weight"].shape[0]
+    subs["img_bev_encoder_neck"] = make_neck_state(n.in_channels, n.embed_dims, len(n.encoder.layers), n.num_heads,
+                                                   n.num_encoder_levels, n.num_points, ffn, seed=seed + 6)
+    order = [k for k in det.state_dict()]
+    flat = {f"{m}.{k}": v for m, s in subs.items() for k, v in s.items()}
+    return {k: flat[k] for k in order if k in flat} | {k: v for k, v in flat.items() if k not in order}
