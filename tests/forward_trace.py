@@ -1,6 +1,7 @@
-"""python tests/forward_trace.py depthnet|r50|b7: one warm CUDA forward under util.trace, then the same forward captured
-into a CUDA graph and replayed.  depthnet: DepthNet at nuScenes R50 shapes; r50: ResNet-50 + SECONDFPN of the nuScenes
-R50 config on (6, 3, 256, 704) images; b7: CustomEfficientNet b7 + SECONDFPN of the KITTI config on (2, 3, 384, 1280)
+"""python tests/forward_trace.py depthnet|r50|r101|b7: one warm CUDA forward under util.trace, then the same forward
+captured with scripts/gpu_bench.graphed and replayed.  depthnet: DepthNet at nuScenes R50 shapes; r50: ResNet-50 +
+SECONDFPN of the nuScenes R50 config on (6, 3, 256, 704) images; r101: ResNetDCN(101) + SECONDFPN of the nuScenes R101
+config on (6, 3, 896, 1600) images; b7: CustomEfficientNet b7 + SECONDFPN of the KITTI config on (2, 3, 384, 1280)
 images.  Run by util.run_trace in a process of its own.  Prints one JSON line: util.trace's counts, whether the replay
 equals eager bit for bit and, for b7, the launch count expected from the module's structure."""
 import json
@@ -16,7 +17,11 @@ from util import images, trace  # noqa: E402
 from occformer_b200 import synth  # noqa: E402
 from occformer_b200.depthnet import DepthNet  # noqa: E402
 from occformer_b200.efficientnet import CustomEfficientNet  # noqa: E402
-from occformer_b200.image_encoder import SECONDFPN, ResNet  # noqa: E402
+from occformer_b200.image_encoder import SECONDFPN, ResNet, ResNetDCN  # noqa: E402
+from scripts.gpu_bench import graphed  # noqa: E402
+
+# the SECONDFPN of the nuScenes R50 and R101 configs
+FPN = dict(in_channels=[256, 512, 1024, 2048], out_channels=[128] * 4, upsample_strides=[0.25, 0.5, 1, 2])
 
 
 def _load(net, state, dev):
@@ -34,10 +39,18 @@ def depthnet(dev):
 
 
 def r50(dev):
-    fpn = dict(in_channels=[256, 512, 1024, 2048], out_channels=[128] * 4, upsample_strides=[0.25, 0.5, 1, 2])
     backbone = _load(ResNet(50), synth.make_resnet_state(seed=30), dev)
-    neck = _load(SECONDFPN(**fpn), synth.make_secondfpn_state(seed=31, **fpn), dev)
+    neck = _load(SECONDFPN(**FPN), synth.make_secondfpn_state(seed=31, **FPN), dev)
     x = images(6, 256, 704, seed=32).to(dev)
+    return lambda: neck(list(backbone(x)))[0], {}
+
+
+def r101(dev):
+    dcn = dict(style="caffe", dcn=dict(type="DCNv2", deform_groups=1, fallback_on_stride=False),
+               stage_with_dcn=(False, False, True, True))
+    backbone = _load(ResNetDCN(101, **dcn), synth.make_resnet_dcn_state(seed=33, **dcn), dev)
+    neck = _load(SECONDFPN(**FPN), synth.make_secondfpn_state(seed=34, **FPN), dev)
+    x = images(6, 896, 1600, seed=35).to(dev)
     return lambda: neck(list(backbone(x)))[0], {}
 
 
@@ -66,17 +79,10 @@ def b7(dev):
 
 @torch.no_grad()
 def main(case):
-    fwd, extra = {"depthnet": depthnet, "r50": r50, "b7": b7}[case](torch.device("cuda:0"))
+    fwd, extra = {"depthnet": depthnet, "r50": r50, "r101": r101, "b7": b7}[case](torch.device("cuda:0"))
     eager = fwd()  # warm-up: weight preparation, module loading, workspaces
     res = dict(trace(fwd), **extra)
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        fwd()  # the side stream's own warm-up (workspaces are per stream)
-    torch.cuda.current_stream().wait_stream(s)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        y = fwd()
+    graph, y = graphed(fwd)
     graph.replay()
     torch.cuda.synchronize()
     res["graph_equals_eager"] = bool(torch.equal(y.view(torch.int32), eager.view(torch.int32)))

@@ -20,14 +20,12 @@ fp32 summation-order accuracy; the outputs are bit for bit when the sums came ou
 """
 import json
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
 
-from util import GOLDEN, HERE, assert_close, f64, images, parity_log
+from util import GOLDEN, assert_close, f64, images, parity_log, run_script
 from vt_chain import check_pooled
 from occformer_b200 import DETECTORS, synth
 
@@ -290,11 +288,7 @@ def test_panoptic_config(cuda):
 
 # ------------------------------------------------------------------ 6. one graph, only library work
 def test_cuda_graph_launch_count_and_kernels(cuda):
-    flags = ["-s"] if sys.flags.no_user_site else []
-    r = subprocess.run([sys.executable, *flags, os.path.join(HERE, "detector_trace.py")], capture_output=True, text=True,
-                       timeout=1200)
-    assert r.returncode == 0, f"detector_trace.py failed:\n{r.stdout[-3000:]}\n{r.stderr[-3000:]}"
-    res = json.loads(r.stdout.strip().splitlines()[-1])
+    res = run_script("detector_trace.py", timeout=1200)
     print(res)
     assert res["counted"] == res["kernels"] + res["memsets"], "the launch counter and the trace disagree"
     assert res["counted"] == sum(res["per_module"].values()), res["per_module"]

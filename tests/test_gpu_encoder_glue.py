@@ -15,58 +15,12 @@ import torch
 
 import encoder_ref as ref
 from oracle import port
-from util import assert_close
+from util import assert_close, launches, rejected, same_bits, sentinel, untouched
+from occformer_b200 import ops
 
 pytestmark = pytest.mark.gpu
 
 GATE, GATE_S32 = ref.GATE_F32, ref.GATE_S32
-SENTINEL = 0x7FC0FFEE  # a NaN: an output row left unwritten also fails the finiteness check of assert_close
-
-
-def _ops():
-    from occformer_b200 import ops
-    return ops
-
-
-def _sentinel(rows, cols, device):
-    return torch.full((rows, cols), SENTINEL, dtype=torch.int32, device=device).view(torch.float32)
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def _same_bits(a, b, what):
-    assert torch.equal(_bits(a), _bits(b)), f"{what}: not bit-identical"
-
-
-def _untouched(t, what):
-    assert bool((_bits(t) == SENTINEL).all()), f"{what}: written outside the output's rows / columns"
-
-
-def _launch(name, *args):
-    """ops._call -> the number of kernels and memsets the entry point enqueued"""
-    ops = _ops()
-    n0 = ops.LAUNCH_COUNT[0]
-    ops._call(name, *args)
-    return ops.LAUNCH_COUNT[0] - n0
-
-
-def _rejected(name, *args, buffers=()):
-    """the call raises, enqueues nothing and leaves every buffer as it was"""
-    ops = _ops()
-    before = [_bits(b).clone() for b in buffers]
-    n0 = ops.LAUNCH_COUNT[0]
-    with pytest.raises(RuntimeError):
-        ops._call(name, *args)
-    torch.cuda.synchronize()
-    assert ops.LAUNCH_COUNT[0] == n0, f"{name}: enqueued work before rejecting the call"
-    for b, b0 in zip(buffers, before):
-        assert torch.equal(_bits(b), b0), f"{name}: a rejected call changed a buffer"
-
-
-def _decode(s):
-    return _ops().unsplit_weight(s)
 
 
 def _dev(cuda, *ts):
@@ -94,7 +48,6 @@ ZMEAN_CASES = [
 
 @pytest.mark.parametrize("B,X,Y,Z,C,groups", ZMEAN_CASES)
 def test_gn_relu_zmean_ln_against_fp64(cuda, B, X, Y, Z, C, groups):
-    ops = _ops()
     XY = X * Y
     nvox, rows = B * XY * Z, B * XY * (Z + 1)
     y, gw, gb = ref.gn_case(B, XY * Z, C, groups)
@@ -104,8 +57,8 @@ def test_gn_relu_zmean_ln_against_fp64(cuda, B, X, Y, Z, C, groups):
     want_tok, want_tokn = ref.gn_relu_zmean_ln(*_d(y), st, *_d(gw, gb, lw, lb), B, XY, Z, groups)
 
     def run(win_shift, tokn_rows):
-        tok, tokn = _sentinel(rows, C, cuda), _sentinel(tokn_rows, C, cuda)
-        n = _launch("occ_gn_relu_zmean_ln", y, st, gw, gb, lw, lb, tok, tokn, B, XY, Z, C, groups, X, win_shift)
+        tok, tokn = sentinel(rows, C, cuda), sentinel(tokn_rows, C, cuda)
+        n = launches("occ_gn_relu_zmean_ln", y, st, gw, gb, lw, lb, tok, tokn, B, XY, Z, C, groups, X, win_shift)
         assert n == 1
         return tok, tokn
 
@@ -113,22 +66,22 @@ def test_gn_relu_zmean_ln_against_fp64(cuda, B, X, Y, Z, C, groups):
     tok, tokn = run(-1, rows)
     assert_close(tok[:nvox], want_tok[:nvox], GATE, f"gn_relu_zmean_ln {case} tok voxel rows")
     assert_close(tok[nvox:], want_tok[nvox:], GATE, f"gn_relu_zmean_ln {case} tok BEV rows")
-    assert_close(_decode(tokn), want_tokn, GATE_S32, f"gn_relu_zmean_ln {case} tokn (S32)")
+    assert_close(ops.unsplit_weight(tokn), want_tokn, GATE_S32, f"gn_relu_zmean_ln {case} tokn (S32)")
     if Z == 1:
-        _same_bits(tok[nvox:], tok[:nvox], "Z = 1: BEV rows vs voxel rows")
+        same_bits(tok[nvox:], tok[:nvox], "Z = 1: BEV rows vs voxel rows")
     tok2, tokn2 = run(-1, rows)
-    _same_bits(tok2, tok, "repeat launch, tok")
-    _same_bits(tokn2, tokn, "repeat launch, tokn")
+    same_bits(tok2, tok, "repeat launch, tok")
+    same_bits(tokn2, tokn, "repeat launch, tokn")
     if C == 128:
         wl_rows = ops.lib().occ_window_layout_rows(B, X, Y, Z)
         for shift in (0, 1):
             tok_w, wl = run(shift, wl_rows)
             idx = ops.window_layout_index(B, X, Y, Z, shift).to(cuda)
-            _same_bits(tok_w, tok, f"win_shift {shift}: tok")
-            _same_bits(wl[idx], tokn, f"win_shift {shift}: window-layout rows vs token order")
+            same_bits(tok_w, tok, f"win_shift {shift}: tok")
+            same_bits(wl[idx], tokn, f"win_shift {shift}: window-layout rows vs token order")
             pad = torch.ones(wl_rows, dtype=torch.bool, device=cuda)
             pad[idx] = False
-            _untouched(wl[pad], f"win_shift {shift}: pad rows of the window layout")
+            untouched(wl[pad], f"win_shift {shift}: pad rows of the window layout")
 
 
 @pytest.mark.parametrize("Z,C,groups", [(17, 128, 32), (4, 384, 32), (4, 128, 64), (13, 1024, 32)])
@@ -138,10 +91,10 @@ def test_gn_relu_zmean_ln_rejects_unsupported_shapes(cuda, Z, C, groups):
     y = torch.randn(B * XY * Z, C, device=cuda)
     st = ref.gn_stats(y.double(), B, groups)
     w, b = torch.ones(C, device=cuda), torch.zeros(C, device=cuda)
-    tok, tokn = _sentinel(rows, C, cuda), _sentinel(rows, C, cuda)
-    _rejected("occ_gn_relu_zmean_ln", y, st, w, b, w, b, tok, tokn, B, XY, Z, C, groups, X, -1, buffers=(tok, tokn))
-    _untouched(tok, "tok")
-    _untouched(tokn, "tokn")
+    tok, tokn = sentinel(rows, C, cuda), sentinel(rows, C, cuda)
+    rejected("occ_gn_relu_zmean_ln", y, st, w, b, w, b, tok, tokn, B, XY, Z, C, groups, X, -1, buffers=(tok, tokn))
+    untouched(tok, "tok")
+    untouched(tokn, "tokn")
 
 
 # ------------------------------------------------------------------------------------------------ occ_layernorm
@@ -150,13 +103,12 @@ def test_gn_relu_zmean_ln_rejects_unsupported_shapes(cuda, Z, C, groups):
 def test_layernorm_against_fp64(cuda, C, rows):
     """C in {128, 256, 512, 1024}: the vectorised kernel; else the generic one (C = 100: lanes with different trip counts,
     fp32 output only).  Eight rows per CTA: 7 and 1001 leave the last CTA partial."""
-    ops = _ops()
     x, w, b = _dev(cuda, ref.ln_input(rows, C, ref.case_seed(rows, C)), *ref.affine(C, ref.case_seed(C)))
     want = ref.layernorm(*_d(x, w, b))
 
     def run(split):
-        out = _sentinel(rows, C, cuda)
-        assert _launch("occ_layernorm", x, w, b, out, rows, C, split) == 1
+        out = sentinel(rows, C, cuda)
+        assert launches("occ_layernorm", x, w, b, out, rows, C, split) == 1
         return out
 
     case = f"C{C} rows{rows}"
@@ -166,12 +118,12 @@ def test_layernorm_against_fp64(cuda, C, rows):
     if special:  # the offset row alone: against its own spread, not the largest value of the tensor
         big = slice(special[2], special[2] + 1)
         assert_close(out[big], want[big], GATE, f"layernorm {case} row offset by 1e3 x its spread")
-    _same_bits(run(0), out, "repeat launch")
+    same_bits(run(0), out, "repeat launch")
     if C % 32 == 0:
         s = run(1)
-        _same_bits(s, ops.to_split(out), "S32 output vs the split of the fp32 output")
-        assert_close(_decode(s), want, GATE_S32, f"layernorm {case} S32")
-        _same_bits(run(1), s, "repeat launch, S32")
+        same_bits(s, ops.to_split(out), "S32 output vs the split of the fp32 output")
+        assert_close(ops.unsplit_weight(s), want, GATE_S32, f"layernorm {case} S32")
+        same_bits(run(1), s, "repeat launch, S32")
 
 
 # ------------------------------------------------------------------------------------------------ occ_gn_apply
@@ -190,7 +142,6 @@ GN_APPLY_CASES = [
 
 @pytest.mark.parametrize("case", GN_APPLY_CASES, ids=lambda c: "B{}-rows{}-C{}-g{}".format(*c[:4]))
 def test_gn_apply_against_fp64(cuda, case):
-    ops = _ops()
     B, rpb, C, groups, with_res, relu, want_f32, ldo, offs = case
     rows = B * rpb
     x, w, b = _dev(cuda, *ref.gn_case(B, rpb, C, groups))
@@ -201,10 +152,10 @@ def test_gn_apply_against_fp64(cuda, case):
     want = ref.gn_apply(*_d(x), st, *_d(w, b), rpb, groups, residual=None if res is None else res.double(), relu=relu)
 
     def run(off):
-        out = _sentinel(rows, C, cuda) if want_f32 else None
-        cat = _sentinel(rows, ldo, cuda) if off is not None else None
-        n = _launch("occ_gn_apply", x, st, w, b, res, out, cat, rows, rpb, C, groups, ldo if cat is not None else C,
-                    off or 0, int(relu))
+        out = sentinel(rows, C, cuda) if want_f32 else None
+        cat = sentinel(rows, ldo, cuda) if off is not None else None
+        n = launches("occ_gn_apply", x, st, w, b, res, out, cat, rows, rpb, C, groups, ldo if cat is not None else C,
+                     off or 0, int(relu))
         assert n == 1
         return out, cat
 
@@ -215,16 +166,16 @@ def test_gn_apply_against_fp64(cuda, case):
             assert_close(out, want, GATE, name)
         if cat is not None:
             sl = cat[:, off:off + C]
-            assert_close(_decode(sl), want, GATE_S32, f"{name} S32 at column {off} of {ldo}")
-            _untouched(cat[:, :off], f"columns before {off}")
-            _untouched(cat[:, off + C:], f"columns after {off + C}")
+            assert_close(ops.unsplit_weight(sl), want, GATE_S32, f"{name} S32 at column {off} of {ldo}")
+            untouched(cat[:, :off], f"columns before {off}")
+            untouched(cat[:, off + C:], f"columns after {off + C}")
             if out is not None:
-                _same_bits(sl, ops.to_split(out), "S32 output vs the split of the fp32 output")
+                same_bits(sl, ops.to_split(out), "S32 output vs the split of the fp32 output")
         if i == 0:
             out2, cat2 = run(off)
             for a, a2 in ((out, out2), (cat, cat2)):
                 if a is not None:
-                    _same_bits(a2, a, "repeat launch")
+                    same_bits(a2, a, "repeat launch")
 
 
 # ------------------------------------------------------------------------------------------------ occ_aspp_gap_branch
@@ -241,15 +192,16 @@ def test_aspp_gap_branch_against_fp64(cuda, B, rpb, ch):
     want = ref.aspp_gap_branch(*_d(x, wconv, gw, gb), B, groups)
     rows, ldo = B * rpb, 5 * ch
     for off in (4 * ch, 0):
-        cat = _sentinel(rows, ldo, cuda)
-        n = _launch("occ_aspp_gap_branch", x, _gap_ws(B, ch, cuda), wconv, gw, gb, cat, B, rpb, ch, groups, ldo, off)
+        cat = sentinel(rows, ldo, cuda)
+        n = launches("occ_aspp_gap_branch", x, _gap_ws(B, ch, cuda), wconv, gw, gb, cat, B, rpb, ch, groups, ldo, off)
         assert n == 4  # memset, column sums, branch, broadcast
         sl = cat[:, off:off + ch]
-        assert_close(_decode(sl), want, GATE_S32, f"aspp_gap_branch B{B} rows{rpb} ch{ch} g{groups} at column {off}")
-        per_sample = _bits(sl).view(B, rpb, ch)
-        assert torch.equal(per_sample, per_sample[:, :1].expand_as(per_sample)), "rows of one sample differ"
-        _untouched(cat[:, :off], f"columns before {off}")
-        _untouched(cat[:, off + ch:], f"columns after {off + ch}")
+        assert_close(ops.unsplit_weight(sl), want, GATE_S32,
+                     f"aspp_gap_branch B{B} rows{rpb} ch{ch} g{groups} at column {off}")
+        per_sample = sl.contiguous().view(B, rpb, ch)
+        same_bits(per_sample, per_sample[:, :1].expand_as(per_sample), "rows of one sample")
+        untouched(cat[:, :off], f"columns before {off}")
+        untouched(cat[:, off + ch:], f"columns after {off + ch}")
 
 
 def test_aspp_gap_branch_rejects_a_slice_past_the_row(cuda):
@@ -257,19 +209,19 @@ def test_aspp_gap_branch_rejects_a_slice_past_the_row(cuda):
     the allocation (columns 32..95 of each 64-float row spill into the next row)"""
     B, rpb, ch, groups = 1, 4, 64, 32
     x, wconv, gw, gb = _dev(cuda, *ref.gap_case(B, rpb, ch, groups))
-    cat = _sentinel(B * rpb + 1, 64, cuda)
-    _rejected("occ_aspp_gap_branch", x, _gap_ws(B, ch, cuda), wconv, gw, gb, cat, B, rpb, ch, groups, 64, 32,
-              buffers=(cat,))
-    _untouched(cat, "concat buffer")
+    cat = sentinel(B * rpb + 1, 64, cuda)
+    rejected("occ_aspp_gap_branch", x, _gap_ws(B, ch, cuda), wconv, gw, gb, cat, B, rpb, ch, groups, 64, 32,
+             buffers=(cat,))
+    untouched(cat, "concat buffer")
 
 
 def test_aspp_gap_branch_rejects_more_than_65535_samples(cuda):
     B, rpb, ch, groups = 65536, 1, 32, 16
     x = torch.randn(B * rpb, ch, device=cuda)
     wconv, gw, gb = torch.randn(ch, ch, device=cuda), torch.ones(ch, device=cuda), torch.zeros(ch, device=cuda)
-    cat = _sentinel(B * rpb, 5 * ch, cuda)
-    _rejected("occ_aspp_gap_branch", x, _gap_ws(B, ch, cuda), wconv, gw, gb, cat, B, rpb, ch, groups, 5 * ch, 4 * ch,
-              buffers=(cat,))
+    cat = sentinel(B * rpb, 5 * ch, cuda)
+    rejected("occ_aspp_gap_branch", x, _gap_ws(B, ch, cuda), wconv, gw, gb, cat, B, rpb, ch, groups, 5 * ch, 4 * ch,
+             buffers=(cat,))
 
 
 # ------------------------------------------------------------------------------------------------ occ_depthnet_gap_branch
@@ -283,28 +235,28 @@ def test_depthnet_gap_branch_against_fp64(cuda, B, rpb, ch):
     rows, ldo, off = B * rpb, ch + 64, 32
 
     def run():
-        cat = _sentinel(rows, ldo, cuda)
+        cat = sentinel(rows, ldo, cuda)
         ws = torch.empty((2, B, ch), dtype=torch.float32, device=cuda)
-        assert _launch("occ_depthnet_gap_branch", x, ws, w, b, cat, B, rpb, ch, ldo, off) == 3
+        assert launches("occ_depthnet_gap_branch", x, ws, w, b, cat, B, rpb, ch, ldo, off) == 3
         return cat
 
     cat = run()
     sl = cat[:, off:off + ch]
-    assert_close(_decode(sl), want, GATE_S32, f"depthnet_gap_branch B{B} rows{rpb} ch{ch}")
-    per_sample = _bits(sl).view(B, rpb, ch)
-    assert torch.equal(per_sample, per_sample[:, :1].expand_as(per_sample)), "rows of one image differ"
-    _untouched(cat[:, :off], "columns before the slice")
-    _untouched(cat[:, off + ch:], "columns after the slice")
-    _same_bits(run(), cat, "repeat launch (fixed-order sums)")
+    assert_close(ops.unsplit_weight(sl), want, GATE_S32, f"depthnet_gap_branch B{B} rows{rpb} ch{ch}")
+    per_sample = sl.contiguous().view(B, rpb, ch)
+    same_bits(per_sample, per_sample[:, :1].expand_as(per_sample), "rows of one image")
+    untouched(cat[:, :off], "columns before the slice")
+    untouched(cat[:, off + ch:], "columns after the slice")
+    same_bits(run(), cat, "repeat launch (fixed-order sums)")
 
 
 # ------------------------------------------------------------------------------------------------ occ_dualpath_fuse
 def _fuse(cuda, x, bev, cw, cbias, identity, split, st, gw, gb, f32, s32, B, XY, Z, C):
     rows = B * XY * Z
-    out = _sentinel(rows, C, cuda) if f32 else None
-    out_s = _sentinel(rows, C, cuda) if s32 else None
-    n = _launch("occ_dualpath_fuse", x, bev, cw, cbias, identity, split, st, gw if st is not None else None,
-                gb if st is not None else None, 32 if st is not None else 0, out, out_s, B, XY, Z, C)
+    out = sentinel(rows, C, cuda) if f32 else None
+    out_s = sentinel(rows, C, cuda) if s32 else None
+    n = launches("occ_dualpath_fuse", x, bev, cw, cbias, identity, split, st, gw if st is not None else None,
+                 gb if st is not None else None, 32 if st is not None else 0, out, out_s, B, XY, Z, C)
     assert n == 1
     return out, out_s
 
@@ -315,13 +267,13 @@ def test_dualpath_fuse_against_fp64(cuda, C, B, XY, Z):
     """every identity kind (S32 block input, fp32, fp32 GroupNorm'd with id_stats) with fp32-only, S32-only and both
     outputs.  (2, 35, 3): 105 rows per sample, so at R = 2 a warp's two rows belong to different samples, and 210 rows
     is not a multiple of 8R."""
-    ops = _ops()
     x, bev, cw, idn = _dev(cuda, *ref.fuse_case(B, XY, Z, C))
     gw, gb = _dev(cuda, *ref.affine(C, ref.case_seed(C, 32)))
     cbias = float(torch.tensor(0.1, dtype=torch.float32))  # the value the kernel receives
     st = ref.gn_stats(idn.double(), B, 32)
     idn_s = ops.to_split(idn)
-    kinds = {"S32": (idn_s, 1, None, _decode(idn_s)), "fp32": (idn, 0, None, idn), "fp32+id_stats": (idn, 0, st, idn)}
+    kinds = {"S32": (idn_s, 1, None, ops.unsplit_weight(idn_s)), "fp32": (idn, 0, None, idn),
+             "fp32+id_stats": (idn, 0, st, idn)}
     for kind, (ident, split, stats, ident_ref) in kinds.items():
         want = ref.dualpath_fuse(*_d(x, bev, cw), cbias, ident_ref.double(), B, XY, Z, id_stats=stats,
                                  id_w=gw.double(), id_b=gb.double(), groups=32)
@@ -332,11 +284,11 @@ def test_dualpath_fuse_against_fp64(cuda, C, B, XY, Z):
             if out is not None:
                 assert_close(out, want, GATE, name)
             if out_s is not None:
-                assert_close(_decode(out_s), want, GATE_S32, f"{name} S32")
-        _same_bits(out_s, ops.to_split(out), "S32 output vs the split of the fp32 output")
+                assert_close(ops.unsplit_weight(out_s), want, GATE_S32, f"{name} S32")
+        same_bits(out_s, ops.to_split(out), "S32 output vs the split of the fp32 output")
         out2, out_s2 = _fuse(*args, 1, 1, B, XY, Z, C)
-        _same_bits(out2, out, "repeat launch")
-        _same_bits(out_s2, out_s, "repeat launch, S32")
+        same_bits(out2, out, "repeat launch")
+        same_bits(out_s2, out_s, "repeat launch, S32")
 
 
 @pytest.mark.parametrize("cbias", [80.0, -80.0])
@@ -355,9 +307,9 @@ def test_dualpath_fuse_saturated_coefficient(cuda, C, cbias):
     out, out_s = _fuse(cuda, x, bev, cw, cbias, idn, 0, None, None, None, 1, 1, B, XY, Z, C)
     assert bool(torch.isfinite(out).all())
     assert_close(out, want, GATE, f"dualpath_fuse C{C} saturated, bias {cbias:+.0f}")
-    _same_bits(out_s, _ops().to_split(out), "S32 output vs the split of the fp32 output")
+    same_bits(out_s, ops.to_split(out), "S32 output vs the split of the fp32 output")
     col = torch.arange(rows, device=cuda) // Z
     one, zero = z > 20, z < -90
     assert int(one.sum() if cbias > 0 else zero.sum()) >= rows // 3
-    _same_bits(out[one], (x + bev[col] + idn)[one], "coefficient exactly 1")
-    _same_bits(out[zero], (x + idn)[zero], "coefficient exactly 0")
+    same_bits(out[one], (x + bev[col] + idn)[one], "coefficient exactly 1")
+    same_bits(out[zero], (x + idn)[zero], "coefficient exactly 0")

@@ -17,58 +17,12 @@ import torch
 
 import neck_ref as ref
 from oracle import port
-from util import assert_close
+from util import assert_close, launches, misaligned, rejected, same_bits, sentinel
+from occformer_b200 import ops
 
 pytestmark = pytest.mark.gpu
 
 GATE, GATE_S32 = ref.GATE_F32, ref.GATE_S32
-SENTINEL = 0x7FC0FFEE  # a NaN: an output row left unwritten fails the finiteness check of assert_close
-
-
-def _ops():
-    from occformer_b200 import ops
-    return ops
-
-
-def _sentinel(rows, cols, device):
-    return torch.full((rows, cols), SENTINEL, dtype=torch.int32, device=device).view(torch.float32)
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32 if t.dtype == torch.float32 else torch.int64)
-
-
-def _same_bits(a, b, what):
-    assert torch.equal(_bits(a), _bits(b)), f"{what}: not bit-identical"
-
-
-def _launch(name, *args):
-    """ops._call -> the number of kernels and memsets the entry point enqueued"""
-    ops = _ops()
-    n0 = ops.LAUNCH_COUNT[0]
-    ops._call(name, *args)
-    return ops.LAUNCH_COUNT[0] - n0
-
-
-def _rejected(name, *args, buffers=(), rc=None):
-    """the call fails (rc -2: returned as unsupported; else raised, as argument error rc when given), enqueues nothing
-    and leaves every buffer as it was"""
-    ops = _ops()
-    before = [_bits(b).clone() for b in buffers]
-    n0 = ops.LAUNCH_COUNT[0]
-    if rc == -2:
-        assert ops._call(name, *args, unsupported_ok=True) == rc
-    else:
-        with pytest.raises(RuntimeError, match=None if rc is None else f"argument error {rc}"):
-            ops._call(name, *args)
-    torch.cuda.synchronize()
-    assert ops.LAUNCH_COUNT[0] == n0, f"{name}: enqueued work before rejecting the call"
-    for b, b0 in zip(buffers, before):
-        assert torch.equal(_bits(b), b0), f"{name}: a rejected call changed a buffer"
-
-
-def _decode(s):
-    return _ops().unsplit_weight(s)
 
 
 def _grids(grids):
@@ -80,16 +34,11 @@ def _strides(strides):
     return (ctypes.c_float * len(strides))(*[float(s) for s in strides])
 
 
-def _misaligned(t):
-    """a view of t's storage starting 4 bytes in (for calls that must reject it before touching it)"""
-    return t.reshape(-1)[1:]
-
-
 # ------------------------------------------------------------------------------------------------ occ_ms_deform_attn
 def _msda(value, ow, grids, strides, B, E, H, head_ld, P=4):
-    out = _sentinel(value.shape[0], E, value.device)
-    n = _launch("occ_ms_deform_attn", value, value.shape[1], head_ld, ow, out, len(grids), B, _grids(grids),
-                _strides(strides), E, H, P)
+    out = sentinel(value.shape[0], E, value.device)
+    n = launches("occ_ms_deform_attn", value, value.shape[1], head_ld, ow, out, len(grids), B, _grids(grids),
+                 _strides(strides), E, H, P)
     assert n == 1
     return out
 
@@ -135,17 +84,17 @@ def test_ms_deform_attn_against_fp64(cuda, case):
             value[:, :, :hd] = base.view(-1, H, hd)
             value = value.view(-1, H * ld)
         out = _msda(value, ow, grids, strides, B, E, H, ld)
-        assert_close(_decode(out), want, GATE_S32, f"{name} head_ld {ld} (S32)")
-        _same_bits(_msda(value, ow, grids, strides, B, E, H, ld), out, f"head_ld {ld}: repeat launch")
+        assert_close(ops.unsplit_weight(out), want, GATE_S32, f"{name} head_ld {ld} (S32)")
+        same_bits(_msda(value, ow, grids, strides, B, E, H, ld), out, f"head_ld {ld}: repeat launch")
         if first is None:
             first = out
         else:
-            _same_bits(out, first, f"head_ld {ld} vs head_ld {lds[0]}")
+            same_bits(out, first, f"head_ld {ld} vs head_ld {lds[0]}")
     if base.shape[0] <= 20000:  # the port's own arithmetic, in fp32 on the host, with its zeros padding
         ow_c = ow.clone()
         n = H * len(grids) * 4 * 3
         ow_c[:, :n] = ow_c[:, :n].clamp(-1e4 - 50, 1e4 + 50)  # grid_sample's int conversion is not defined at 1e30
-        got = _decode(_msda(base, ow_c, grids, strides, B, E, H, hd))
+        got = ops.unsplit_weight(_msda(base, ow_c, grids, strides, B, E, H, hd))
         assert_close(got, _port_fp32(base, ow_c, grids, strides, B, E, H, hd), GATE_S32, f"{name} vs the fp32 port")
 
 
@@ -163,7 +112,7 @@ def test_ms_deform_attn_rejects(cuda, what):
     hd = E // H
     value = torch.randn(rows, E, device=cuda)
     ow = torch.randn(rows, H * len(grids) * 4 * 4, device=cuda)
-    out = _sentinel(rows, E, cuda)
+    out = sentinel(rows, E, cuda)
     ld, v = hd, value
     if what == "P3":
         P = 3
@@ -172,10 +121,10 @@ def test_ms_deform_attn_rejects(cuda, what):
         value = torch.randn(rows, E - 4, device=cuda)
         v = value
     elif what == "value_misaligned":
-        v = _misaligned(value)
+        v = misaligned(value)
     rc = -2 if what == "P3" else -1
-    _rejected("occ_ms_deform_attn", v, value.shape[1], ld, ow, out, len(grids), B, _grids(grids), _strides(strides), E,
-              H, P, buffers=(out, value, ow), rc=rc)
+    rejected("occ_ms_deform_attn", v, value.shape[1], ld, ow, out, len(grids), B, _grids(grids), _strides(strides), E,
+             H, P, buffers=(out, value, ow), rc=rc)
 
 
 # ------------------------------------------------------------------------------------------------ occ_neck_token_prep
@@ -188,7 +137,6 @@ _COMBOS = [(f, s, p) for f in (0, 1) for s in (0, 1) for p in (0, 1) if f or s o
 def test_token_prep_against_fp64(cuda, C, L, B):
     """with and without the LayerNorm; all seven output combinations give the same bits for the outputs present;
     out_s32 = split(out_f32) and out_pos = split(out_f32 + pos[start_l + local]) bit for bit"""
-    ops = _ops()
     grids = ref.TOKEN_GRIDS[L]
     x, pos = ref.token_input(grids, B, C, ref.case_seed(C, L, B))
     lw, lb = ref.affine(C, ref.case_seed(C))
@@ -202,14 +150,15 @@ def test_token_prep_against_fp64(cuda, C, L, B):
         name = f"token_prep C{C} L{L} B{B} {'LN' if ln else 'no LN'}"
         outs = {}
         for f, s, p in _COMBOS:
-            o = [_sentinel(rows, C, cuda) if w else None for w in (f, s, p)]
-            n = _launch("occ_neck_token_prep", x, *(ln or (None, None)), pos if p else None, *o, L, B, _grids(grids), C)
+            o = [sentinel(rows, C, cuda) if w else None for w in (f, s, p)]
+            n = launches("occ_neck_token_prep", x, *(ln or (None, None)), pos if p else None, *o, L, B, _grids(grids),
+                         C)
             assert n == 1
             for k, t in enumerate(o):
                 if t is None:
                     continue
                 if k in outs:
-                    _same_bits(t, outs[k], f"{name}: output {k} with outputs {(f, s, p)}")
+                    same_bits(t, outs[k], f"{name}: output {k} with outputs {(f, s, p)}")
                 else:
                     outs[k] = t
         f32, s32, ps = outs[0], outs[1], outs[2]
@@ -220,10 +169,10 @@ def test_token_prep_against_fp64(cuda, C, L, B):
             low = slice(special[0], special[0] + 1)
             assert_close(f32[low], want[low], GATE, f"{name}: row with variance near 1e-4")
         if ln is None:
-            _same_bits(f32, x, f"{name}: out_f32 without the LayerNorm is the input")
-        _same_bits(s32, ops.to_split(f32), f"{name}: S32 output vs the split of the fp32 output")
-        _same_bits(ps, ops.to_split(f32 + pos[idx]), f"{name}: out_pos vs split(out_f32 + pos[start_l + local])")
-        assert_close(_decode(ps), want_pos, GATE_S32, f"{name} x + pos (S32)")
+            same_bits(f32, x, f"{name}: out_f32 without the LayerNorm is the input")
+        same_bits(s32, ops.to_split(f32), f"{name}: S32 output vs the split of the fp32 output")
+        same_bits(ps, ops.to_split(f32 + pos[idx]), f"{name}: out_pos vs split(out_f32 + pos[start_l + local])")
+        assert_close(ops.unsplit_weight(ps), want_pos, GATE_S32, f"{name} x + pos (S32)")
 
 
 @pytest.mark.parametrize("what", ["C160", "ln_w_without_ln_b", "out_pos_without_pos"])
@@ -233,13 +182,13 @@ def test_token_prep_rejects(cuda, what):
     rows = B * sum(x * y * z for x, y, z in grids)
     x, pos = torch.randn(rows, C, device=cuda), torch.randn(rows, C, device=cuda)
     w, b = torch.ones(C, device=cuda), torch.zeros(C, device=cuda)
-    outs = [_sentinel(rows, C, cuda) for _ in range(3)]
+    outs = [sentinel(rows, C, cuda) for _ in range(3)]
     if what == "ln_w_without_ln_b":
         b = None
     if what == "out_pos_without_pos":
         pos = None
-    _rejected("occ_neck_token_prep", x, w, b, pos, *outs, len(grids), B, _grids(grids), C, buffers=outs,
-              rc=-2 if what == "C160" else -1)
+    rejected("occ_neck_token_prep", x, w, b, pos, *outs, len(grids), B, _grids(grids), C, buffers=outs,
+             rc=-2 if what == "C160" else -1)
 
 
 # ------------------------------------------------------------------------------------------------ occ_gn_upsample_add
@@ -254,8 +203,8 @@ def _gn_up_case(case, device):
 def _gn_up(cur, st, gw, gb, groups, coarse):
     B, X, Y, Z, C = cur.shape
     _, Xc, Yc, Zc, _ = coarse.shape
-    out = _sentinel(B * X * Y * Z, C, cur.device).view(cur.shape)
-    n = _launch("occ_gn_upsample_add", cur, st, gw, gb, groups, coarse, out, B, X, Y, Z, Xc, Yc, Zc, C)
+    out = sentinel(B * X * Y * Z, C, cur.device).view(cur.shape)
+    n = launches("occ_gn_upsample_add", cur, st, gw, gb, groups, coarse, out, B, X, Y, Z, Xc, Yc, Zc, C)
     assert n == 1
     return out
 
@@ -274,13 +223,13 @@ def test_gn_upsample_add_against_fp64(cuda, case):
     want = ref.gn_upsample_add(cur.double(), st, gw.double(), gb.double(), groups, coarse.double())
     name = f"gn_upsample_add B{B} {X}x{Y}x{Z} from {tuple(coarse.shape[1:4])} C{C} g{groups}"
     out = _gn_up(cur, st, gw, gb, groups, coarse)
-    got = _decode(out.view(-1, C)).view(cur.shape)
+    got = ops.unsplit_weight(out.view(-1, C)).view(cur.shape)
     assert_close(got, want, GATE_S32, f"{name} (S32)")
     cpg = C // groups
     for b, gi in ref.gn_special(B, groups):
         sl = (b, Ellipsis, slice(gi * cpg, (gi + 1) * cpg))
         assert_close(got[sl], want[sl], GATE_S32, f"{name}: sample {b} group {gi} (mean / std = 100)")
-    _same_bits(_gn_up(cur, st, gw, gb, groups, coarse), out, "repeat launch")
+    same_bits(_gn_up(cur, st, gw, gb, groups, coarse), out, "repeat launch")
 
 
 @pytest.mark.parametrize("which", ["cur", "coarse", "out_s"])
@@ -290,11 +239,11 @@ def test_gn_upsample_add_rejects_misaligned_tensors(cuda, which):
     B, X, Y, Z, C = cur.shape
     _, Xc, Yc, Zc, _ = coarse.shape
     st = ref.gn_stats(cur.view(-1, C), B, 32)
-    out = _sentinel(B * X * Y * Z + 1, C, cuda)
+    out = sentinel(B * X * Y * Z + 1, C, cuda)
     args = {"cur": cur, "coarse": coarse, "out_s": out}
-    args[which] = _misaligned(args[which])
-    _rejected("occ_gn_upsample_add", args["cur"], st, gw, gb, 32, args["coarse"], args["out_s"], B, X, Y, Z, Xc, Yc, Zc,
-              C, buffers=(out, cur, coarse))
+    args[which] = misaligned(args[which])
+    rejected("occ_gn_upsample_add", args["cur"], st, gw, gb, 32, args["coarse"], args["out_s"], B, X, Y, Z, Xc, Yc, Zc,
+             C, buffers=(out, cur, coarse))
 
 
 # ------------------------------------------------------------------------------------------------ occ_gn_stats
@@ -310,7 +259,7 @@ def test_gn_stats_against_fp64(cuda, case):
     want_st = ref.gn_stats(x, B, groups)
     prior = torch.randn(B, groups, 2, generator=torch.Generator().manual_seed(case), dtype=torch.float64).to(cuda)
     st = prior.clone()
-    assert _launch("occ_gn_stats", x, st, B, rows, C, cpg) == 1
+    assert launches("occ_gn_stats", x, st, B, rows, C, cpg) == 1
     got_st = st - prior
     name = f"gn_stats B{B} rows{rows} C{C} cpg{cpg}"
     n = rows * cpg
@@ -344,4 +293,4 @@ def test_gn_stats_rejects(cuda, what):
         cpg = 5
     x = torch.randn(B * rows, C, device=cuda)
     st = torch.zeros(B, max(1, C // cpg), 2, dtype=torch.float64, device=cuda)
-    _rejected("occ_gn_stats", _misaligned(x) if what == "x_misaligned" else x, st, B, rows, C, cpg, buffers=(st,))
+    rejected("occ_gn_stats", misaligned(x) if what == "x_misaligned" else x, st, B, rows, C, cpg, buffers=(st,))

@@ -11,13 +11,13 @@ import pytest
 import torch
 
 import neck_ref as ref
-from util import assert_close
+from util import assert_close, graph_replay, same_bits
+from occformer_b200 import ops
 
 pytestmark = pytest.mark.gpu
 
 GATE = 5e-5        # fp32 outputs and decoded S32 outputs vs fp64 (four chained contractions and two LayerNorms)
 GATE_BF16 = 3e-2   # single-pass bf16 mode vs fp64
-SENTINEL = 0x7FC0FFEE  # a NaN: an output row left unwritten fails the finiteness check of assert_close
 NUSC_200 = [(25, 25, 2), (50, 50, 4), (100, 100, 8)]
 # (grids, B, E, F)
 CASES = {
@@ -28,19 +28,6 @@ CASES = {
     "E96_L3_B2": (ref.TOKEN_GRIDS[3], 2, 96, 192),
 }
 _COMBOS = [(f, s, p) for f in (0, 1) for s in (0, 1) for p in (0, 1) if f or s or p]
-
-
-def _ops():
-    from occformer_b200 import ops
-    return ops
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def _same_bits(a, b, what):
-    assert torch.equal(_bits(a), _bits(b)), f"{what}: not bit-identical"
 
 
 def _layer_norm(y, w, b, eps=ref.EPS):
@@ -61,7 +48,6 @@ def tail_ref(att, x, wo, bo, ln1, w1, b1, w2, b2, ln2, pos_rows):
 
 def _case(name, device):
     """inputs of a case: S32 operands (att, wo, w1, w2) plus their decoded values, the rest fp32"""
-    ops = _ops()
     grids, B, E, F = CASES[name]
     seed = ref.case_seed(len(grids), B, E, F)
     x, pos = ref.token_input(grids, B, E, seed)
@@ -87,7 +73,6 @@ def _case(name, device):
 
 def _run(c, want_f32=True, want_s32=True, want_pos=True):
     """one call of ops.neck_layer_tail -> (outputs, library launches it enqueued)"""
-    ops = _ops()
     n0 = ops.LAUNCH_COUNT[0]
     out = ops.neck_layer_tail(c["att_s"], c["x"], c["wo_s"], c["bo"], c["ln1"], c["w1_s"], c["b1"], c["w2_s"], c["b2"],
                               c["ln2"], c["grids"], c["B"], pos=c["pos"], want_f32=want_f32, want_s32=want_s32,
@@ -96,7 +81,6 @@ def _run(c, want_f32=True, want_s32=True, want_pos=True):
 
 
 def _want(c):
-    ops = _ops()
     dec = ops.unsplit_weight
     return tail_ref(dec(c["att_s"]), c["x"], dec(c["wo_s"]), c["bo"], c["ln1"], dec(c["w1_s"]), c["b1"], dec(c["w2_s"]),
                     c["b2"], c["ln2"], c["pos_rows"])
@@ -104,7 +88,6 @@ def _want(c):
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_neck_layer_tail_against_fp64(cuda, name):
-    ops = _ops()
     c = _case(name, cuda)
     want, want_pos = _want(c)
     outs = {}
@@ -116,7 +99,7 @@ def test_neck_layer_tail_against_fp64(cuda, name):
             if t is None:
                 continue
             if k in outs:
-                _same_bits(t, outs[k], f"{name}: output {k} with outputs {combo}")
+                same_bits(t, outs[k], f"{name}: output {k} with outputs {combo}")
             else:
                 outs[k] = t
     f32, s32, ps = outs[0], outs[1], outs[2]
@@ -125,30 +108,20 @@ def test_neck_layer_tail_against_fp64(cuda, name):
     if c["special"]:
         big = slice(c["special"][2], c["special"][2] + 1)
         assert_close(f32[big], want[big], GATE, f"{name}: row offset by 1e3 x its spread")
-    _same_bits(s32, ops.to_split(f32), f"{name}: S32 output vs the split of the fp32 output")
-    _same_bits(ps, ops.to_split(f32 + c["pos_rows"]), f"{name}: pos output vs split(out + pos[start_l + local])")
+    same_bits(s32, ops.to_split(f32), f"{name}: S32 output vs the split of the fp32 output")
+    same_bits(ps, ops.to_split(f32 + c["pos_rows"]), f"{name}: pos output vs split(out + pos[start_l + local])")
     # repeats and a CUDA-graph replay give the same bits
     again, _ = _run(c)
     for a, b in zip(again, (f32, s32, ps)):
-        _same_bits(a, b, f"{name}: repeat")
-    stream = torch.cuda.Stream()
-    stream.wait_stream(torch.cuda.current_stream())
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.stream(stream):
-        with torch.cuda.graph(graph, stream=stream):
-            captured, _ = _run(c)
-    torch.cuda.current_stream().wait_stream(stream)
-    for t in captured:
-        t.fill_(float("nan"))
-    graph.replay()
-    torch.cuda.synchronize()
+        same_bits(a, b, f"{name}: repeat")
+    captured = []
+    graph_replay(lambda: captured.extend(_run(c)[0]), captured)
     for a, b in zip(captured, (f32, s32, ps)):
-        _same_bits(a, b, f"{name}: CUDA-graph replay")
+        same_bits(a, b, f"{name}: CUDA-graph replay")
 
 
 @pytest.mark.parametrize("name", ["nusc200_B1", "E96_L3_B2"])
 def test_neck_layer_tail_bf16_mode(cuda, name):
-    ops = _ops()
     c = _case(name, cuda)
     want, want_pos = _want(c)
     with ops.precision("bf16"):
@@ -164,7 +137,6 @@ _BAD = ["E160", "F48", "att_rows", "w2_shape", "att_f64", "pos_missing", "rows_v
 @pytest.mark.parametrize("what", _BAD)
 def test_neck_layer_tail_rejects(cuda, what):
     """bad shapes and dtypes fail on the host: nothing is enqueued"""
-    ops = _ops()
     grids, B = ref.TOKEN_GRIDS[3], 1
     E, F = (160, 640) if what == "E160" else (192, 48 if what == "F48" else 768)
     rows = B * sum(x * y * z for x, y, z in grids)

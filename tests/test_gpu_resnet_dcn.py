@@ -1,17 +1,15 @@
 """ResNetDCN on the library's kernels (image_encoder.py ResNetDCN._bottleneck_cuda): the modulated deformable im2col one
 launch at a time against an fp64 restatement of mmcv's sampling, the DCN Bottlenecks, the whole R101-DCN at the nuScenes
-R101 size, the chain images -> R101-DCN -> SECONDFPN -> view transformer, the launch count and CUDA-graph replay, the
-shape contract and the bf16 mode.  The module oracle is image_encoder.py's torch forward in float64 on the GPU (pinned
-on the host by tests/test_cpu_resnet_dcn.py)."""
+R101 size, the chain images -> R101-DCN -> SECONDFPN -> view transformer, the launch count and CUDA-graph replay
+(tests/forward_trace.py r101, in a process of its own), the shape contract and the bf16 mode.  The module oracle is
+image_encoder.py's torch forward in float64 on the GPU (pinned on the host by tests/test_cpu_resnet_dcn.py)."""
 import json
 import os
-import subprocess
-import sys
 
 import pytest
 import torch
 
-from util import GOLDEN, HERE, assert_close, bits, f64, images, parity_log, rel_err, rel_rms
+from util import GOLDEN, assert_close, bits, f64, images, parity_log, rel_err, rel_rms, run_trace
 from vt_chain import check_pooled
 from occformer_b200 import BACKBONES, NECKS, ops, synth
 from occformer_b200.common import twin_of
@@ -55,20 +53,6 @@ def r101_view_transformer(seed, B):
     sd["bn.running_var"] = mlp.reshape(-1, dn.cam_channels).var(0, unbiased=False) + 1.0
     dn.load_state_dict(sd, strict=True)
     return vt.eval(), cams, mlp
-
-
-def run_r101_trace(timeout):
-    """tests/resnet_dcn_trace.py in a process of its own (as util.run_trace runs tests/forward_trace.py): its profiler
-    session and graph capture stay out of this process.  Asserts that the forward ran only library kernels.  -> its
-    result"""
-    flags = ["-s"] if sys.flags.no_user_site else []
-    r = subprocess.run([sys.executable, *flags, os.path.join(HERE, "resnet_dcn_trace.py")], capture_output=True,
-                       text=True, timeout=timeout)
-    assert r.returncode == 0, f"resnet_dcn_trace.py failed:\n{r.stdout}\n{r.stderr}"
-    res = json.loads(r.stdout.strip().splitlines()[-1])
-    print(f"[r101 launches] counted {res['counted']}, trace: {res['kernels']} occ:: kernels + {res['memsets']} memsets")
-    assert not res["other"], f"non-library GPU work: {res['other'][:5]}"
-    return res
 
 
 def ref_modulated_cols(x, off, n, H, W):
@@ -238,7 +222,7 @@ def test_images_to_view_transformer(cuda):
 
 # ------------------------------------------------------------------ 5. only library kernels, graph-safe
 def test_only_library_kernels_and_cuda_graph(cuda):
-    res = run_r101_trace(1500)
+    res = run_trace("r101", 1500)
     assert res["memsets"] == 0
     # stem im2col + GEMM + max-pool, 33 Bottlenecks x (3 convs + split) + 4 downsamples, 26 DCNs x (conv_offset +
     # modulated im2col), SECONDFPN: 2 space_to_depth + 3 convs + GEMM + depth_to_space

@@ -28,82 +28,15 @@ import pytest
 import torch
 
 import swin_ref as ref
-from util import assert_close, parity_log, rel_err
+from util import (assert_close, graph_replay, launches, misaligned, parity_log, rejected, rel_err, same_bits,
+                  sentinel, untouched)
+from occformer_b200 import ops
 
 pytestmark = pytest.mark.gpu
 
 GATE = ref.GATE
-SENTINEL = 0x7FC0FFEE  # a NaN: an output row left unwritten also fails the finiteness check of assert_close
 WA_STAGES = 4          # csrc/window_geom.cuh: units in flight per CTA of window_attn_tc_kernel
 EXTRA_ROWS = 3         # sentinel rows behind every output
-
-
-def _ops():
-    from occformer_b200 import ops
-    return ops
-
-
-def _sentinel(rows, cols, device):
-    return torch.full((rows, cols), SENTINEL, dtype=torch.int32, device=device).view(torch.float32)
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def _same_bits(a, b, what):
-    assert torch.equal(_bits(a), _bits(b)), f"{what}: not bit-identical"
-
-
-def _untouched(t, what):
-    assert bool((_bits(t) == SENTINEL).all()), f"{what}: written outside the output's rows"
-
-
-def _launch(name, *args):
-    """ops._call -> the number of kernels and memsets the entry point enqueued"""
-    ops = _ops()
-    n0 = ops.LAUNCH_COUNT[0]
-    ops._call(name, *args)
-    return ops.LAUNCH_COUNT[0] - n0
-
-
-def _rejected(name, *args, buffers=(), unsupported=False):
-    """the call raises (or, unsupported, returns -2 under unsupported_ok), enqueues nothing and changes no buffer"""
-    ops = _ops()
-    before = [_bits(b).clone() for b in buffers]
-    n0 = ops.LAUNCH_COUNT[0]
-    if unsupported:
-        assert ops._call(name, *args, unsupported_ok=True) == -2
-    else:
-        with pytest.raises(RuntimeError):
-            ops._call(name, *args)
-    torch.cuda.synchronize()
-    assert ops.LAUNCH_COUNT[0] == n0, f"{name}: enqueued work before rejecting the call"
-    for b, b0 in zip(buffers, before):
-        assert torch.equal(_bits(b), b0), f"{name}: a rejected call changed a buffer"
-
-
-def _graph_replay(fn, out):
-    """fn() launched inside a captured CUDA graph, replayed into a cleared out -> out after the replay"""
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.stream(s):
-        with torch.cuda.graph(graph, stream=s):
-            fn()
-    torch.cuda.current_stream().wait_stream(s)
-    out.view(torch.int32).fill_(SENTINEL)
-    graph.replay()
-    torch.cuda.synchronize()
-    return out
-
-
-def _s32(t):
-    return _ops().split_weight(t)
-
-
-def _dec(t):
-    return _ops().unsplit_weight(t).double()
 
 
 def _sm_count():
@@ -130,22 +63,22 @@ def _wa(cuda, B, X, Y, Z, C, shift):
     """-> (run(head_major) -> S32 output slice of a sentinel buffer, fp64 reference, plants)"""
     heads = C // ref.HD
     qkv, b, table, plants = ref.qkv_case(B, X, Y, Z, C, shift, ref.case_seed(B, X, Y, Z))
-    qkv_s, b_s = _s32(qkv.to(cuda)), _s32(b.view(1, -1).to(cuda)).view(-1)
+    qkv_s, b_s = ops.split_weight(qkv.to(cuda)), ops.split_weight(b.view(1, -1).to(cuda)).view(-1)
     bias = ref.bias_pad(table).to(cuda)
-    want = ref.window_attention(_dec(qkv_s), _dec(b_s.view(1, -1)).view(-1), table.double().to(cuda), B, X, Y, Z, C,
-                                heads, shift)
+    qkv_d, b_d = ops.unsplit_weight(qkv_s).double(), ops.unsplit_weight(b_s.view(1, -1)).view(-1).double()
+    want = ref.window_attention(qkv_d, b_d, table.double().to(cuda), B, X, Y, Z, C, heads, shift)
     # head-major order moves whole 32-column S32 chunks: [q|k|v][head] -> [head][q|k|v]
     hm = qkv_s.view(-1, 3, heads, 32).permute(0, 2, 1, 3).reshape(qkv_s.shape[0], 3 * C).contiguous()
     hm_b = b_s.view(3, heads, 32).permute(1, 0, 2).reshape(-1).contiguous()
     rows = qkv.shape[0]
 
     def run(head_major=False):
-        buf = _sentinel(rows + EXTRA_ROWS, C, cuda)
+        buf = sentinel(rows + EXTRA_ROWS, C, cuda)
         out = buf[:rows]
         a, bb = (hm, hm_b) if head_major else (qkv_s, b_s)
-        n = _launch("occ_window_attention", a, bb, bias, out, B, X, Y, Z, C, heads, int(shift), int(head_major))
+        n = launches("occ_window_attention", a, bb, bias, out, B, X, Y, Z, C, heads, int(shift), int(head_major))
         assert n == 1, f"{n} launches"
-        _untouched(buf[rows:], "rows past the output")
+        untouched(buf[rows:], "rows past the output")
         return out
 
     return run, want, plants, (qkv_s, b_s, bias)
@@ -158,13 +91,13 @@ def test_window_attention_geometry(cuda, B, X, Y, Z, shift):
     run, want, plants, _ = _wa(cuda, B, X, Y, Z, C, shift)
     out = run()
     case = f"B{B} {X}x{Y}x{Z} shift={int(shift)} ({ref.n_windows(B, X, Y, Z)} windows)"
-    assert_close(_dec(out), want, GATE, f"window_attention {case}")
+    assert_close(ops.unsplit_weight(out), want, GATE, f"window_attention {case}")
     for name in ("large", "onehot", "pad", "uniform"):
         r = _window_rows(B, X, Y, Z, shift, name, plants, cuda)
         if r.numel():
-            assert_close(_dec(out[r]), want[r], GATE, f"window_attention {case} {name} window")
-    _same_bits(run(), out, "repeat launch")
-    _same_bits(run(head_major=True), out, "head-major vs reference qkv order")
+            assert_close(ops.unsplit_weight(out[r]), want[r], GATE, f"window_attention {case} {name} window")
+    same_bits(run(), out, "repeat launch")
+    same_bits(run(head_major=True), out, "head-major vs reference qkv order")
 
 
 def _wrap_shapes():
@@ -182,10 +115,10 @@ def test_window_attention_stage_shapes_wrap_the_ring(cuda, B, X, Y, Z, C):
     for shift in (True, False):
         run, want, _, _ = _wa(cuda, B, X, Y, Z, C, shift)
         out = run()
-        assert_close(_dec(out), want, GATE, f"window_attention C{C} B{B} {X}x{Y}x{Z} shift={int(shift)} ({units} units "
-                                            "per CTA)")
+        assert_close(ops.unsplit_weight(out), want, GATE,
+                     f"window_attention C{C} B{B} {X}x{Y}x{Z} shift={int(shift)} ({units} units per CTA)")
         if shift:
-            _same_bits(run(head_major=True), out, "head-major vs reference qkv order")
+            same_bits(run(head_major=True), out, "head-major vs reference qkv order")
 
 
 def test_window_attention_graph_replay_and_bf16(cuda):
@@ -195,30 +128,29 @@ def test_window_attention_graph_replay_and_bf16(cuda):
     out = run()
     rows = out.shape[0]
     g_out = torch.empty_like(out)
-    replay = _graph_replay(lambda: _ops()._call("occ_window_attention", qkv_s, b_s, bias, g_out, B, X, Y, Z, C, C // 32,
-                                                1, 0), g_out)
-    _same_bits(replay, out, "CUDA-graph replay")
-    with _ops().precision("bf16"):
+    graph_replay(lambda: ops._call("occ_window_attention", qkv_s, b_s, bias, g_out, B, X, Y, Z, C, C // 32, 1, 0),
+                 [g_out])
+    same_bits(g_out, out, "CUDA-graph replay")
+    with ops.precision("bf16"):
         low = run()
     assert rows == low.shape[0]
-    assert_close(_dec(low), want, ref.BF16_GATE, "window_attention single-pass bf16")
+    assert_close(ops.unsplit_weight(low), want, ref.BF16_GATE, "window_attention single-pass bf16")
 
 
 # ------------------------------------------------------------------------------------------------ occ_swin_qkv_attention
 def _fused(cuda, B, X, Y, Z, shift):
     """-> (run(pad_fill=None) -> S32 output slice of a sentinel buffer, fp64 reference, plants, decoded fp64 qkv + bias,
     launch arguments)"""
-    ops = _ops()
     C, heads = 128, 4
     tok, w, b, table, plants = ref.token_case(B, X, Y, Z, shift, ref.case_seed(B, X, Y, Z))
     perm = ref.head_major_perm(C, heads).to(cuda)
-    tok_s = _s32(tok.to(cuda))
-    w_hm = _s32(w.to(cuda)[perm])
+    tok_s = ops.split_weight(tok.to(cuda))
+    w_hm = ops.split_weight(w.to(cuda)[perm])
     b_hm = b.to(cuda)[perm].contiguous()
     w_ref = torch.empty(3 * C, C, dtype=torch.float64, device=cuda)
-    w_ref[perm] = _dec(w_hm)
+    w_ref[perm] = ops.unsplit_weight(w_hm).double()
     b_ref = b.double().to(cuda)
-    tok_d = _dec(tok_s)
+    tok_d = ops.unsplit_weight(tok_s).double()
     table_d = table.double().to(cuda)
     want, pv = ref.qkv_attention(tok_d, w_ref, b_ref, table_d, B, X, Y, Z, C, heads, shift, split_qkv=True,
                                  with_abs=True)
@@ -227,11 +159,11 @@ def _fused(cuda, B, X, Y, Z, shift):
     rows = tok.shape[0]
 
     def run(tokens=wl):
-        buf = _sentinel(rows + EXTRA_ROWS, C, cuda)
+        buf = sentinel(rows + EXTRA_ROWS, C, cuda)
         out = buf[:rows]
-        n = _launch("occ_swin_qkv_attention", tokens, w_hm, b_hm, bias, out, B, X, Y, Z, C, heads, int(shift))
+        n = launches("occ_swin_qkv_attention", tokens, w_hm, b_hm, bias, out, B, X, Y, Z, C, heads, int(shift))
         assert n == 1, f"{n} launches"
-        _untouched(buf[rows:], "rows past the output")
+        untouched(buf[rows:], "rows past the output")
         return out
 
     return run, want, plants, (ref.s32(tok_d @ w_ref.T + b_ref), ref.s32(b_ref), pv), (wl, w_hm, b_hm, bias)
@@ -253,7 +185,7 @@ def _judge_fused(out, want, qkv_d, b_d, pv, plants, B, X, Y, Z, shift, case):
     large = _window_rows(B, X, Y, Z, shift, "large", plants, dev)
     rest = torch.ones(out.shape[0], dtype=torch.bool, device=dev)
     rest[large] = False
-    got = _dec(out)
+    got = ops.unsplit_weight(out).double()
     _assert_pv_close(got[rest], want[rest], pv[rest], f"swin_qkv_attention {case}")
     for name in ("onehot", "pad", "uniform"):
         r = _window_rows(B, X, Y, Z, shift, name, plants, dev)
@@ -277,7 +209,7 @@ def test_swin_qkv_attention_geometry(cuda, B, X, Y, Z, shift):
     out = run()
     case = f"B{B} {X}x{Y}x{Z} shift={int(shift)} ({ref.n_windows(B, X, Y, Z)} windows)"
     _judge_fused(out, want, qkv_d, b_d, pv, plants, B, X, Y, Z, shift, case)
-    _same_bits(run(), out, "repeat launch")
+    same_bits(run(), out, "repeat launch")
     if (B, X, Y, Z) == (1, 200, 200, 16):
         assert _units_per_cta(ref.n_windows(B, X, Y, Z), 4) > 2
 
@@ -289,9 +221,9 @@ def test_swin_qkv_attention_ignores_window_padding_rows(cuda, B, X, Y, Z, shift)
     out = run()
     filled = wl.clone().view(-1, 64, 128)
     g = torch.Generator(device=wl.device).manual_seed(5)
-    filled[:, ref.WT:] = _s32(torch.randn(filled.shape[0] * 15, 128, generator=g, device=wl.device) * 3 + 1).view(-1, 15,
-                                                                                                              128)
-    _same_bits(run(filled.view_as(wl)), out, "window layout with non-zero MMA padding rows")
+    pad = torch.randn(filled.shape[0] * 15, 128, generator=g, device=wl.device) * 3 + 1
+    filled[:, ref.WT:] = ops.split_weight(pad).view(-1, 15, 128)
+    same_bits(run(filled.view_as(wl)), out, "window layout with non-zero MMA padding rows")
 
 
 def test_swin_qkv_attention_graph_replay_and_bf16(cuda):
@@ -299,32 +231,33 @@ def test_swin_qkv_attention_graph_replay_and_bf16(cuda):
     run, want, plants, _, (wl, w_hm, b_hm, bias) = _fused(cuda, B, X, Y, Z, True)
     out = run()
     g_out = torch.empty_like(out)
-    replay = _graph_replay(lambda: _ops()._call("occ_swin_qkv_attention", wl, w_hm, b_hm, bias, g_out, B, X, Y, Z, 128,
-                                                4, 1), g_out)
-    _same_bits(replay, out, "CUDA-graph replay")
-    with _ops().precision("bf16"):
+    graph_replay(lambda: ops._call("occ_swin_qkv_attention", wl, w_hm, b_hm, bias, g_out, B, X, Y, Z, 128, 4, 1),
+                 [g_out])
+    same_bits(g_out, out, "CUDA-graph replay")
+    with ops.precision("bf16"):
         low = run()
     # the large-logit window is left out: a single bf16 pass moves its ~97 scores by ~0.4
     keep = torch.ones(out.shape[0], dtype=torch.bool, device=cuda)
     keep[_window_rows(B, X, Y, Z, True, "large", plants, cuda)] = False
-    assert_close(_dec(low)[keep], want[keep], ref.BF16_GATE, "swin_qkv_attention single-pass bf16")
+    assert_close(ops.unsplit_weight(low)[keep], want[keep], ref.BF16_GATE, "swin_qkv_attention single-pass bf16")
 
 
 # ------------------------------------------------------------------------------------------------ occ_swin_proj_ffn
 def _tail(cuda, M):
     att, tok, wp, bp, lw, lb, w1, b1, w2, b2 = (t.to(cuda) for t in ref.tail_case(M, ref.case_seed(M)))
-    att_s, wp_s, w1_s, w2_s = (_s32(t) for t in (att, wp, w1, w2))
-    want = ref.swin_tail(_dec(att_s), tok.double(), _dec(wp_s), bp.double(), lw.double(), lb.double(), _dec(w1_s),
-                         b1.double(), _dec(w2_s), b2.double())
-    y1 = tok.double() + _dec(att_s) @ _dec(wp_s).T + bp.double()
+    att_s, wp_s, w1_s, w2_s = (ops.split_weight(t) for t in (att, wp, w1, w2))
+    att_d, wp_d, w1_d, w2_d = (ops.unsplit_weight(t).double() for t in (att_s, wp_s, w1_s, w2_s))
+    want = ref.swin_tail(att_d, tok.double(), wp_d, bp.double(), lw.double(), lb.double(), w1_d, b1.double(), w2_d,
+                         b2.double())
+    y1 = tok.double() + att_d @ wp_d.T + bp.double()
     args = (att_s, tok, wp_s, bp, lw, lb, w1_s, b1, w2_s, b2)
 
     def run():
-        buf = _sentinel(M + EXTRA_ROWS, 128, cuda)
+        buf = sentinel(M + EXTRA_ROWS, 128, cuda)
         out = buf[:M]
-        n = _launch("occ_swin_proj_ffn", *args, out, M, 128)
+        n = launches("occ_swin_proj_ffn", *args, out, M, 128)
         assert n == 1, f"{n} launches"
-        _untouched(buf[M:], "rows past the output")
+        untouched(buf[M:], "rows past the output")
         return out
 
     return run, want, y1 + b2.double(), args
@@ -352,7 +285,7 @@ def test_swin_proj_ffn_against_fp64(cuda, M):
         parity_log(f"[parity] swin_proj_ffn M={M} row offset by 1e3: max err {err:.2e} = {err / ulp:.1f} ulp "
                    f"(allowed {allowed:.2e})")
         assert err <= allowed, f"offset row: max error {err:.3e} > {allowed:.3e}"
-    _same_bits(run(), out, "repeat launch")
+    same_bits(run(), out, "repeat launch")
 
 
 def test_swin_proj_ffn_graph_replay_and_bf16(cuda):
@@ -360,68 +293,62 @@ def test_swin_proj_ffn_graph_replay_and_bf16(cuda):
     run, want, _, args = _tail(cuda, M)
     out = run()
     g_out = torch.empty_like(out)
-    _same_bits(_graph_replay(lambda: _ops()._call("occ_swin_proj_ffn", *args, g_out, M, 128), g_out), out,
-               "CUDA-graph replay")
-    with _ops().precision("bf16"):
+    graph_replay(lambda: ops._call("occ_swin_proj_ffn", *args, g_out, M, 128), [g_out])
+    same_bits(g_out, out, "CUDA-graph replay")
+    with ops.precision("bf16"):
         low = run()
     assert_close(low, want, ref.BF16_GATE, "swin_proj_ffn single-pass bf16")
 
 
 # ------------------------------------------------------------------------------------------------ rejections
-def _misaligned(rows, cols, device):
-    """a (rows, cols) fp32 tensor 4 bytes past a 16-byte boundary, inside an allocation one float longer"""
-    return torch.zeros(rows * cols + 4, device=device)[1:1 + rows * cols].view(rows, cols)
-
-
 def test_window_attention_rejects_bad_arguments(cuda):
     B, X, Y, Z, C, heads = 1, 7, 7, 1, 128, 4
     rows = B * X * Y * (Z + 1)
     qkv, b = torch.zeros(rows, 3 * C, device=cuda), torch.zeros(3 * C, device=cuda)
-    bias, out = torch.zeros(heads * 8, ref.BIAS_FLOATS, device=cuda), _sentinel(rows, C, cuda)
+    bias, out = torch.zeros(heads * 8, ref.BIAS_FLOATS, device=cuda), sentinel(rows, C, cuda)
     name = "occ_window_attention"
-    _rejected(name, qkv, b, bias, out, B, X, Y, Z, C, 3, 1, 0, buffers=(out,))              # C != heads * 32
-    _rejected(name, _misaligned(rows, 3 * C, cuda), b, bias, out, B, X, Y, Z, C, heads, 1, 0, buffers=(out,))
-    _rejected(name, qkv, b, bias, _misaligned(rows, C, cuda), B, X, Y, Z, C, heads, 1, 0)
+    rejected(name, qkv, b, bias, out, B, X, Y, Z, C, 3, 1, 0, buffers=(out,))               # C != heads * 32
+    rejected(name, misaligned(qkv), b, bias, out, B, X, Y, Z, C, heads, 1, 0, buffers=(out,))
+    rejected(name, qkv, b, bias, misaligned(out), B, X, Y, Z, C, heads, 1, 0, buffers=(out,))
     r0 = B * X * Y
-    _rejected(name, qkv[:r0], b, bias, out[:r0], B, X, Y, 0, C, heads, 1, 0, buffers=(out,))  # Z = 0
+    rejected(name, qkv[:r0], b, bias, out[:r0], B, X, Y, 0, C, heads, 1, 0, buffers=(out,))   # Z = 0
     h = _sm_count() + 1                                                                         # more heads than SMs
     qkv_h, b_h = torch.zeros(rows, 3 * 32 * h, device=cuda), torch.zeros(3 * 32 * h, device=cuda)
-    bias_h, out_h = torch.zeros(h, ref.BIAS_FLOATS, device=cuda), _sentinel(rows, 32 * h, cuda)
-    _rejected(name, qkv_h, b_h, bias_h, out_h, B, X, Y, Z, 32 * h, h, 1, 0, buffers=(out_h,))
+    bias_h, out_h = torch.zeros(h, ref.BIAS_FLOATS, device=cuda), sentinel(rows, 32 * h, cuda)
+    rejected(name, qkv_h, b_h, bias_h, out_h, B, X, Y, Z, 32 * h, h, 1, 0, buffers=(out_h,))
 
 
 def test_swin_qkv_attention_rejects_bad_arguments(cuda):
     """(more heads than SMs cannot be asked of it: C = 128 fixes four heads)"""
-    ops = _ops()
     B, X, Y, Z, C, heads = 1, 7, 7, 1, 128, 4
     rows = B * X * Y * (Z + 1)
     wl_rows = ops.lib().occ_window_layout_rows(B, X, Y, Z)
     wl, w, b = torch.zeros(wl_rows, C, device=cuda), torch.zeros(3 * C, C, device=cuda), torch.zeros(3 * C, device=cuda)
-    bias, out = torch.zeros(8, ref.BIAS_FLOATS, device=cuda), _sentinel(rows, C, cuda)
+    bias, out = torch.zeros(8, ref.BIAS_FLOATS, device=cuda), sentinel(rows, C, cuda)
     name = "occ_swin_qkv_attention"
-    _rejected(name, wl, w, b, bias, out, B, X, Y, Z, C, 3, 1, buffers=(out,))                # C != heads * 32
-    _rejected(name, _misaligned(wl_rows, C, cuda), w, b, bias, out, B, X, Y, Z, C, heads, 1, buffers=(out,))
-    _rejected(name, wl, w, b, bias, _misaligned(rows, C, cuda), B, X, Y, Z, C, heads, 1)
+    rejected(name, wl, w, b, bias, out, B, X, Y, Z, C, 3, 1, buffers=(out,))                 # C != heads * 32
+    rejected(name, misaligned(wl), w, b, bias, out, B, X, Y, Z, C, heads, 1, buffers=(out,))
+    rejected(name, wl, w, b, bias, misaligned(out), B, X, Y, Z, C, heads, 1, buffers=(out,))
     r0 = B * X * Y
-    _rejected(name, wl, w, b, bias, out[:r0], B, X, Y, 0, C, heads, 1, buffers=(out,))       # Z = 0
+    rejected(name, wl, w, b, bias, out[:r0], B, X, Y, 0, C, heads, 1, buffers=(out,))        # Z = 0
     C2 = 256                                                                                   # C != 128: unsupported
     wl2, w2, b2 = torch.zeros(wl_rows, C2, device=cuda), torch.zeros(3 * C2, C2, device=cuda), torch.zeros(3 * C2,
                                                                                                      device=cuda)
-    out2 = _sentinel(rows, C2, cuda)
-    _rejected(name, wl2, w2, b2, bias, out2, B, X, Y, Z, C2, 8, 1, buffers=(out2,), unsupported=True)
+    out2 = sentinel(rows, C2, cuda)
+    rejected(name, wl2, w2, b2, bias, out2, B, X, Y, Z, C2, 8, 1, buffers=(out2,), rc=-2)
 
 
 def test_swin_proj_ffn_rejects_bad_arguments(cuda):
     M, C = 200, 128
     att, tok = torch.zeros(M, C, device=cuda), torch.zeros(M, C, device=cuda)
     w, v = torch.zeros(C, C, device=cuda), torch.zeros(C, device=cuda)
-    out = _sentinel(M, C, cuda)
+    out = sentinel(M, C, cuda)
     name = "occ_swin_proj_ffn"
-    _rejected(name, att, tok, w, v, v, v, w, v, w, v, out, 0, C, buffers=(out,))  # M = 0
-    _rejected(name, _misaligned(M, C, cuda), tok, w, v, v, v, w, v, w, v, out, M, C, buffers=(out,))
-    _rejected(name, att, tok, w, v, v, v, w, v, w, v, _misaligned(M, C, cuda), M, C)
+    rejected(name, att, tok, w, v, v, v, w, v, w, v, out, 0, C, buffers=(out,))  # M = 0
+    rejected(name, misaligned(att), tok, w, v, v, v, w, v, w, v, out, M, C, buffers=(out,))
+    rejected(name, att, tok, w, v, v, v, w, v, w, v, misaligned(out), M, C, buffers=(out,))
     C2 = 256                                                                                   # C != 128: unsupported
     att2, tok2, w2, v2 = (torch.zeros(M, C2, device=cuda), torch.zeros(M, C2, device=cuda),
                           torch.zeros(C2, C2, device=cuda), torch.zeros(C2, device=cuda))
-    out2 = _sentinel(M, C2, cuda)
-    _rejected(name, att2, tok2, w2, v2, v2, v2, w2, v2, w2, v2, out2, M, C2, buffers=(out2,), unsupported=True)
+    out2 = sentinel(M, C2, cuda)
+    rejected(name, att2, tok2, w2, v2, v2, v2, w2, v2, w2, v2, out2, M, C2, buffers=(out2,), rc=-2)
