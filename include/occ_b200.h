@@ -466,6 +466,28 @@ int occ_panoptic_eval(const long long* x_sem, const long long* x_inst, const lon
                       long long n, int K, unsigned int ignore_mask, int min_points, int parts, void* ws,
                       size_t ws_bytes, long long* state, occ_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * Occupancy ground truth from the labelled LiDAR points (csrc/occ_targets.cu): the gt_occ of
+ *   LoadNuscOccupancyAnnotations          P/datasets/pipelines/loading_nusc_occ.py:95-138 (nb_process_label :122-138)
+ *   LoadNuscPanopticOccupancyAnnotations  P/datasets/pipelines/loading_nusc_panoptic_occ.py:120-166 (nb_process_label :147-166)
+ * built from the points_occ the test loop already hands to the model.  pts (n, ld >= 4) fp32 rows [x, y, z, label, ...]
+ * of B samples, sample b at rows [offsets[b], offsets[b+1]); offsets = B + 1 HOST int64, offsets[0] = 0, non-decreasing,
+ * 1 <= B <= 256.  Voxel index floor((clip(p, lo, hi - 1e-5) - lo) / voxel_size) in float64, voxel_size = (hi - lo) / grid
+ * computed on the host as numpy does.  Each occupied voxel takes its majority id (ties: the smallest id, np.argmax), then
+ * 0 -> ignore and empty_id -> 0; unoccupied voxels are 0.  panoptic = 0: ids < 256, every id votes.  panoptic = 1: ids
+ * < 65536, id 0 does not vote (a voxel holding only id 0 becomes ignore) except in the voxel that comes last in
+ * np.lexsort((x, y, z)) order (largest z, then y, then x) of its sample, where the reference's counter keeps it.
+ * out (B, X, Y, Z) int64, overwritten.  Points with a label that is negative, not an integer or >= the mode's limit, or
+ * with a non-finite coordinate, and (voxel, id) pairs of more than 65535 points (the reference's uint16 counter wraps)
+ * add to *invalid (one device int, ACCUMULATED) and are never written out of bounds.  n = 0 gives an all-zero volume.
+ * ws: occ_lidarseg_occupancy_workspace_bytes(n, B) bytes, 16-byte aligned, zeroed by the call.  Five enqueued launches /
+ * memsets per call, deterministic (integer atomics only), no host synchronisation. */
+size_t occ_lidarseg_occupancy_workspace_bytes(long long n, int B);
+int occ_lidarseg_occupancy(const float* pts, int ld, const long long* offsets /*HOST*/, int B, double x_min,
+                           double y_min, double z_min, double x_max, double y_max, double z_max, int X, int Y, int Z,
+                           int panoptic, long long empty_id, long long ignore, int* invalid, void* ws, size_t ws_bytes,
+                           long long* out, occ_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -3,7 +3,7 @@
 Registry names / constructor kwargs / forward signatures / state_dict keys follow
 projects/mmdet3d_plugin of the reference; all arithmetic runs in csrc/libocc_b200.so (C ABI, ctypes).
 """
-from .registry import ATTENTION, BACKBONES, DETECTORS, HEADS, NECKS, POSITIONAL_ENCODING  # noqa: F401
+from .registry import ATTENTION, BACKBONES, DETECTORS, HEADS, NECKS, PIPELINES, POSITIONAL_ENCODING  # noqa: F401
 from .encoder import DualpathTransformerBlock, OccupancyEncoder  # noqa: F401
 from .image_encoder import SECONDFPN, ResNet, ResNetDCN  # noqa: F401
 from .efficientnet import CustomEfficientNet  # noqa: F401
@@ -12,5 +12,6 @@ from .neck import MSDeformAttnPixelDecoder3D, MultiScaleDeformableAttention3D  #
 from .head import (Mask2FormerNuscOccHead, Mask2FormerNuscPanopticOccHead, Mask2FormerOccHead,  # noqa: F401
                    SinePositionalEncoding3D)
 from .detector import OccupancyFormer  # noqa: F401
+from .pipelines import LoadNuscOccupancyPoints, LoadNuscPanopticOccupancyPoints  # noqa: F401
 
 __version__ = "0.1.0"

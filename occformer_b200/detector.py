@@ -23,8 +23,8 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import dist_eval
-from .head import Mask2FormerNuscPanopticOccHead
+from . import dist_eval, targets
+from .head import Mask2FormerNuscOccHead, Mask2FormerNuscPanopticOccHead
 from .image_encoder import SECONDFPN, ResNet, ResNetDCN
 from .registry import BACKBONES, DETECTORS, HEADS, NECKS
 
@@ -52,8 +52,13 @@ class OccupancyFormer(nn.Module):
     def __init__(self, img_view_transformer, img_bev_encoder_backbone, img_bev_encoder_neck, pts_voxel_layer=None,
                  pts_voxel_encoder=None, pts_middle_encoder=None, pts_fusion_layer=None, img_backbone=None,
                  pts_backbone=None, img_neck=None, pts_neck=None, pts_bbox_head=None, img_roi_head=None,
-                 img_rpn_head=None, train_cfg=None, test_cfg=None, pretrained=None, init_cfg=None):
+                 img_rpn_head=None, train_cfg=None, test_cfg=None, pretrained=None, init_cfg=None,
+                 occ_targets_from_points=False):
+        """occ_targets_from_points (not a reference kwarg): simple_test called without gt_occ builds 'target_voxels' from
+        points_occ on the GPU (occupancy_targets), for a pipeline whose loader skips the host-side ground truth
+        (occformer_b200.pipelines, INTEGRATION.md)."""
         super().__init__()
+        self.occ_targets_from_points = bool(occ_targets_from_points)
         lidar = dict(pts_voxel_layer=pts_voxel_layer, pts_voxel_encoder=pts_voxel_encoder,
                      pts_middle_encoder=pts_middle_encoder, pts_backbone=pts_backbone, pts_fusion_layer=pts_fusion_layer,
                      pts_neck=pts_neck, img_rpn_head=img_rpn_head, img_roi_head=img_roi_head)
@@ -145,6 +150,8 @@ class OccupancyFormer(nn.Module):
         The panoptic head's dict is returned as the head makes it, plus 'target_voxels' and 'target_points': its
         'output_voxels' is [(semantic, panoptic)] and its 'output_points' are labels already, which the reference detector
         cannot take (INTEGRATION.md)."""
+        if gt_occ is None and points_occ is not None and self.occ_targets_from_points:
+            gt_occ = self.occupancy_targets(points_occ, img_metas)
         voxel_feats, img_feats, depth = self.extract_feat(points=None, img=img, img_metas=img_metas)
         output = self.pts_bbox_head.simple_test(voxel_feats=voxel_feats, points=points_occ, img_metas=img_metas,
                                                 img_feats=img_feats, points_uv=points_uv)
@@ -163,6 +170,27 @@ class OccupancyFormer(nn.Module):
         output["output_voxels"] = output["output_voxels"][0]
         output["target_voxels"] = gt_occ
         return output
+
+    def occupancy_targets(self, points_occ, img_metas, unoccupied_id=17):
+        """The gt_occ the reference's nuScenes loader builds for these points (occformer_b200.targets), on their device:
+        points_occ = list of per-sample (n_i, 4) CUDA tensors [x, y, z, label | panoptic id], occ_size and pc_range from
+        img_metas[0] -> int64 (B, X, Y, Z): semantic labels for Mask2FormerNuscOccHead, panoptic ids for
+        Mask2FormerNuscPanopticOccHead.  Reads one invalid-point count back to the host (ValueError if nonzero)."""
+        head = self.pts_bbox_head
+        if isinstance(head, Mask2FormerNuscPanopticOccHead):
+            build = targets.panoptic_occupancy
+        elif isinstance(head, Mask2FormerNuscOccHead):
+            build = targets.lidarseg_occupancy
+        else:
+            raise NotImplementedError(f"occupancy_targets: {type(head).__name__} scores against preprocessed voxel labels "
+                                      "(SemanticKITTI), not a LiDAR point scan; pass gt_occ")
+        # the reference's datasets store both fields as numpy arrays (nuscenes_lss_dataset.py:86-87), configs as lists
+        occ_size, pc_range = (np.asarray(img_metas[0][k]) for k in ("occ_size", "pc_range"))
+        same = (np.array_equal(np.asarray(m["occ_size"]), occ_size) and np.array_equal(np.asarray(m["pc_range"]), pc_range)
+                for m in img_metas[1:])
+        if not all(same):
+            raise ValueError("occupancy_targets: every sample of a batch needs the same occ_size and pc_range")
+        return build(list(points_occ), [int(v) for v in occ_size], [float(v) for v in pc_range], unoccupied_id)
 
     def post_process_semantic(self, pred_occ):
         """occupancyformer.py:239-244: class of the largest softmax probability, (B, K, ...) -> (B, ...).  An evaluation

@@ -939,3 +939,35 @@ def lidarseg_hist(scores, labels, K, hist=None):
         hist = torch.zeros((K - 1, K - 1), dtype=torch.int64, device=scores.device)
     _call("occ_lidarseg_hist", scores, labels, scores.shape[0], K, hist)
     return hist
+
+
+# ----------------------------------------------------------------------------------------------- occupancy ground truth
+_targets_ws = {}  # (device, stream) -> grow-only uint8 workspace of occ_lidarseg_occupancy
+
+
+def lidarseg_occupancy(pts, counts, pc_range, grid, panoptic, empty_id, ignore):
+    """Occupancy ground truth of B samples (occ_lidarseg_occupancy): pts (n, ld >= 4) fp32 CUDA rows [x, y, z, label, ...],
+    sample b the next counts[b] rows -> (int64 (B, X, Y, Z) volume, int32 (1,) invalid-point counter); no synchronisation."""
+    B = len(counts)
+    n, ld = pts.shape
+    offsets = [0]
+    for c in counts:
+        offsets.append(offsets[-1] + int(c))
+    assert offsets[-1] == n
+    X, Y, Z = (int(v) for v in grid)
+    dev = pts.device
+    nbytes = lib().occ_lidarseg_occupancy_workspace_bytes(n, B)
+    if nbytes == 0:
+        raise RuntimeError(f"occformer_b200: occ_lidarseg_occupancy takes 1..256 samples and at most 2^30 points, "
+                           f"got {B} samples, {n} points")
+    key = (str(dev), torch.cuda.current_stream(dev).cuda_stream)
+    ws = _targets_ws.get(key)
+    if ws is None or ws.numel() < nbytes:
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        _targets_ws[key] = ws
+    out = torch.empty((B, X, Y, Z), dtype=torch.int64, device=dev)
+    invalid = torch.zeros(1, dtype=torch.int32, device=dev)
+    r = [float(v) for v in pc_range]
+    _call("occ_lidarseg_occupancy", pts, ld, (ctypes.c_longlong * (B + 1))(*offsets), B, *r, X, Y, Z, int(panoptic),
+          int(empty_id), int(ignore), invalid, ws, ws.numel(), out)
+    return out, invalid

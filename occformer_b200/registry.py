@@ -95,3 +95,6 @@ HEADS = _Mirror("head", [("mmdet.models.builder", "HEADS"), ("mmdet3d.models.bui
 POSITIONAL_ENCODING = _Mirror("position encoding", [("mmcv.cnn.bricks.registry", "POSITIONAL_ENCODING"),
                                                     ("mmcv.cnn.bricks.transformer", "POSITIONAL_ENCODING")])
 ATTENTION = _Mirror("attention", [("mmcv.cnn.bricks.registry", "ATTENTION"), ("mmcv.cnn.bricks.transformer", "ATTENTION")])
+# loader transforms (mmdet 2.x keeps the registry in mmdet.datasets.builder, where the reference registers its loaders,
+# P/datasets/pipelines/loading_nusc_occ.py:9,13)
+PIPELINES = _Mirror("pipeline", [("mmdet.datasets.builder", "PIPELINES")])
