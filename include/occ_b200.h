@@ -488,6 +488,35 @@ int occ_lidarseg_occupancy(const float* pts, int ld, const long long* offsets /*
                            int panoptic, long long empty_id, long long ignore, int* invalid, void* ws, size_t ws_bytes,
                            long long* out, occ_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * Camera images from the decoded frames (csrc/image_prep.cu): steps 2-4 of the test loaders' image side,
+ *   LoadMultiViewImageFromFiles_OccFormer     P/datasets/pipelines/loading_nusc_imgs.py:34-62,181-195
+ *   LoadMultiViewImageFromFiles_SemanticKitti P/datasets/pipelines/loading_kitti_imgs.py:35-65
+ * bit for bit: Pillow 9.4's Image.resize((rW, rH)) (BICUBIC, a = -0.5, no reducing_gap) of the uint8 BGR frame, then
+ * Image.crop((x0, y0, x0 + fW, y0 + fH)) (0 outside the resized image), then mmcv's imnormalize as a table lookup.
+ * Resize: separable, horizontal pass first; each pass accumulates (1 << 21) + sum w * p in int32 over Pillow's
+ * precompute_coeffs taps (weights normalised in float64, then int32 with 22 fractional bits, rounded away from zero) and
+ * clips >> 22 to [0, 255]; the horizontal result is uint8.  An unchanged axis gives identity weights, i.e. Pillow's copy.
+ * Only the source rows and resized columns the crop needs are computed.
+ *   frames     uint8, frame_bytes bytes; image m is HWC BGR at byte offsets[m] (HOST int64), H x W x 3 bytes
+ *   geom       HOST int32 (M, 6): H, W, rW, rH, x0, y0 per image
+ *   tables     HOST int64 (M, 2): device addresses of image m's horizontal (W -> rW) and vertical (H -> rH) tables,
+ *              each int32 [2 * n] (first tap, tap count) per output index, then [ksize * n] weights tap-major
+ *              (w[k * n + i]), n = rW | rH, ksize = 2 * ceil(2 * max(in / n, 1)) + 1 (Pillow's; unused taps 0)
+ *   norm       device float (3, 256): output channel c of source value v = norm[c * 256 + v]; swap_rb = 1 reads output
+ *              channel c from source channel 2 - c (BGR -> RGB), swap_rb = 0 from channel c
+ *   out        float (M, 3, fH, fW), overwritten
+ *   ws         occ_prepare_images_workspace_bytes(geom, M, fH, fW) bytes (the uint8 horizontal-pass rows), 16-byte
+ *              aligned; 0 bytes when no crop overlaps its resized image
+ * 1 <= M <= 256.  Two kernel launches per call whatever M and the geometries, no memset, no host synchronisation.
+ * Returns -1 for: M out of range, a non-positive size, a frame past frame_bytes, a crop origin with |x0|, |y0| >= 2^30,
+ * a null table, a short or misaligned workspace, swap_rb not 0 / 1.  Returns -2 when an axis needs more than 129 taps
+ * (a downscale by more than 32), the bound of the kernels' shared-memory row span.  Nothing is enqueued on an error. */
+size_t occ_prepare_images_workspace_bytes(const int* geom /*HOST*/, int M, int fH, int fW);
+int occ_prepare_images(const unsigned char* frames, long long frame_bytes, const long long* offsets /*HOST*/,
+                       const int* geom /*HOST*/, int M, int fH, int fW, const long long* tables /*HOST*/,
+                       const float* norm, int swap_rb, void* ws, size_t ws_bytes, float* out, occ_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -12,6 +12,7 @@ from .neck import MSDeformAttnPixelDecoder3D, MultiScaleDeformableAttention3D  #
 from .head import (Mask2FormerNuscOccHead, Mask2FormerNuscPanopticOccHead, Mask2FormerOccHead,  # noqa: F401
                    SinePositionalEncoding3D)
 from .detector import OccupancyFormer  # noqa: F401
-from .pipelines import LoadNuscOccupancyPoints, LoadNuscPanopticOccupancyPoints  # noqa: F401
+from .pipelines import (LoadMultiViewImageFrames_OccFormer, LoadMultiViewImageFrames_SemanticKitti,  # noqa: F401
+                        LoadNuscOccupancyPoints, LoadNuscPanopticOccupancyPoints)
 
 __version__ = "0.1.0"

@@ -23,7 +23,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import dist_eval, targets
+from . import dist_eval, image_prep, targets
 from .head import Mask2FormerNuscOccHead, Mask2FormerNuscPanopticOccHead
 from .image_encoder import SECONDFPN, ResNet, ResNetDCN
 from .registry import BACKBONES, DETECTORS, HEADS, NECKS
@@ -113,8 +113,18 @@ class OccupancyFormer(nn.Module):
 
     def extract_img_feat(self, img, img_metas):
         """img = [imgs, rots, trans, intrins, post_rots, post_trans, bda, ...] -> (voxel_feats list, depth, img_feats).
-        The reference clones the image features for a head that ignores them; they are handed on as they are."""
-        x = self.image_encoder(img[0])
+        The reference clones the image features for a head that ignores them; they are handed on as they are.
+        imgs may also be the uint8 (B, N, H, W, 3) BGR frames of occformer_b200.pipelines' LoadMultiViewImageFrames_*
+        transforms: they are resized, cropped and normalised on the GPU first (image_prep.prepare_images), from the
+        'img_aug' of each sample's metas."""
+        imgs = img[0]
+        if (imgs.dtype if torch.is_tensor(imgs) else imgs[0].dtype) == torch.uint8:
+            if img_metas is None or any("img_aug" not in m for m in img_metas):
+                raise ValueError("OccupancyFormer: uint8 camera frames need each sample's 'img_aug' meta, which the "
+                                 "LoadMultiViewImageFrames_OccFormer / LoadMultiViewImageFrames_SemanticKitti transforms "
+                                 "produce; add 'img_aug' to Collect3D's meta_keys")
+            imgs = image_prep.prepare_images(imgs, [m["img_aug"] for m in img_metas])
+        x = self.image_encoder(imgs)
         img_feats = x
         rots, trans, intrins, post_rots, post_trans, bda = img[1:7]
         mlp_input = self.img_view_transformer.get_mlp_input(rots, trans, intrins, post_rots, post_trans, bda)

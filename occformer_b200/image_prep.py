@@ -1,0 +1,118 @@
+"""Camera images on the GPU from the decoded frames: the resize, crop and normalisation of the reference's test loaders
+(LoadMultiViewImageFromFiles_OccFormer, P/datasets/pipelines/loading_nusc_imgs.py:34-62,181-195;
+LoadMultiViewImageFromFiles_SemanticKitti, loading_kitti_imgs.py:35-65), bit for bit (csrc/image_prep.cu).
+
+The loader transforms of occformer_b200.pipelines hand the model uint8 BGR frames and, per sample, an ``img_aug`` meta:
+
+    {"resize_dims": [[rW, rH], ...], "crop": [[x0, y0, x1, y1], ...],   # one per camera, as sample_augmentation gives
+     "input_size": [fH, fW], "mean": [3 floats], "std": [3 floats], "to_rgb": bool}   # mmlabNormalize's config
+
+The host part here is table building: Pillow's bicubic coefficients per (source size, resized size) of an axis and the
+normalisation as a 3 x 256 table, both in float64 numpy, one operation at a time as x86-64 builds of Pillow and OpenCV
+compute them (no fused multiply-add).  ops.prepare_images caches them on the device.
+"""
+import math
+
+import numpy as np
+import torch
+
+from . import ops
+
+PRECISION_BITS = 22  # Pillow's resample.c: 32 - 8 - 2
+DEFAULT_NORM = dict(mean=[123.675, 116.28, 103.53], std=[58.395, 57.12, 57.375], to_rgb=True)  # mmlabNormalize's
+
+
+def _bicubic(x):
+    """Pillow's bicubic_filter, a = -0.5, in its operation order"""
+    x = np.abs(x)
+    a = -0.5
+    near = ((a + 2.0) * x - (a + 3.0)) * x * x + 1
+    far = (((x - 5) * x + 8) * x - 4) * a
+    return np.where(x < 1.0, near, np.where(x < 2.0, far, 0.0))
+
+
+def resample_table(in_size, out_size):
+    """Pillow's precompute_coeffs + normalize_coeffs_8bpc for one axis of Image.resize (box (0, in_size)) -> int32
+    [2 * out_size] (first tap, tap count per output index) ++ [ksize * out_size] weights tap-major, 22 fractional bits"""
+    scale = float(in_size) / out_size
+    filterscale = max(scale, 1.0)
+    support = 2.0 * filterscale
+    ksize = int(math.ceil(support)) * 2 + 1
+    center = (np.arange(out_size) + 0.5) * scale
+    first = np.maximum(np.trunc(center - support + 0.5).astype(np.int64), 0)
+    last = np.minimum(np.trunc(center + support + 0.5).astype(np.int64), in_size)
+    count = last - first
+    ss = 1.0 / filterscale
+    taps = np.arange(ksize)
+    w = _bicubic(((taps[None, :] + first[:, None]) - center[:, None] + 0.5) * ss)
+    w = np.where(taps[None, :] < count[:, None], w, 0.0)
+    ww = np.zeros(out_size)
+    for k in range(ksize):  # the C loop's order, not numpy's pairwise sum
+        ww = ww + w[:, k]
+    w = np.where(ww[:, None] != 0.0, w / np.where(ww == 0.0, 1.0, ww)[:, None], w)
+    fixed = w * (1 << PRECISION_BITS)
+    fixed = np.trunc(np.where(w < 0, -0.5 + fixed, 0.5 + fixed)).astype(np.int32)
+    bounds = np.stack([first, count], axis=1).astype(np.int32)
+    return np.concatenate([bounds.reshape(-1), fixed.T.reshape(-1)])
+
+
+def normalize_table(mean, std, to_rgb):
+    """mmcv's imnormalize of every uint8 value -> float32 (3, 256) in output channel order: cv2.subtract of the float64
+    mean, rounded to float32, then cv2.multiply by the float64 1 / std, rounded to float32.  to_rgb (cvtColor BGR2RGB
+    first) leaves the table as it is: output channel c then reads source channel 2 - c (the kernel's swap_rb)."""
+    mean = np.asarray(mean, dtype=np.float32).astype(np.float64)
+    stdinv = 1 / np.asarray(std, dtype=np.float32).astype(np.float64)
+    v = np.arange(256, dtype=np.float64)
+    rows = [((v - mean[c]).astype(np.float32).astype(np.float64) * stdinv[c]).astype(np.float32) for c in range(3)]
+    return np.stack(rows)
+
+
+def norm_config(img_norm_cfg):
+    """mmlabNormalize's reading of img_norm_cfg (None: its defaults) -> dict(mean, std, to_rgb) of plain Python values"""
+    cfg = DEFAULT_NORM if img_norm_cfg is None else img_norm_cfg
+    return dict(mean=[float(v) for v in cfg["mean"]], std=[float(v) for v in cfg["std"]], to_rgb=bool(cfg["to_rgb"]))
+
+
+def prepare_images(frames, img_aug):
+    """frames: uint8 CUDA (B, N, H, W, 3) BGR, or a list of B per-sample (N, H_i, W_i, 3) tensors; img_aug: B metas (the
+    module docstring) -> float32 (B, N, 3, fH, fW), the reference loaders' img_inputs[0] stacked by the collate.
+    All samples must share input_size and the normalisation config."""
+    if torch.is_tensor(frames):
+        if frames.dim() != 5:
+            raise ValueError(f"prepare_images: frames must be (B, N, H, W, 3), got {tuple(frames.shape)}")
+        samples = list(frames.unbind(0))
+    else:
+        samples = list(frames)
+    if len(samples) != len(img_aug) or not samples:
+        raise ValueError(f"prepare_images: {len(samples)} samples of frames but {len(img_aug)} img_aug metas")
+    for s in samples:
+        if s.dtype != torch.uint8 or s.dim() != 4 or s.shape[-1] != 3:
+            raise ValueError(f"prepare_images: every sample must be uint8 (N, H, W, 3), got {s.dtype} "
+                             f"{tuple(s.shape)}")
+        if not s.is_cuda:
+            raise RuntimeError("prepare_images: frames must be CUDA tensors (no CPU fallback exists)")
+    a0 = img_aug[0]
+    size = [int(v) for v in a0["input_size"]]
+    norm = norm_config(a0)
+    N = samples[0].shape[0]
+    for s, a in zip(samples, img_aug):
+        if [int(v) for v in a["input_size"]] != size or norm_config(a) != norm:
+            raise ValueError("prepare_images: every sample of a batch needs the same input_size and normalisation")
+        if s.shape[0] != N or len(a["resize_dims"]) != N or len(a["crop"]) != N:
+            raise ValueError("prepare_images: every sample needs the same number of cameras, one resize and crop each")
+        for (rW, rH), (x0, y0, x1, y1) in zip(a["resize_dims"], a["crop"]):
+            if (int(x1) - int(x0), int(y1) - int(y0)) != (size[1], size[0]):
+                raise ValueError(f"prepare_images: crop {(x0, y0, x1, y1)} is not input_size {tuple(size)}")
+    if torch.is_tensor(frames) and frames.is_contiguous():
+        flat = frames.reshape(-1)
+    else:
+        flat = torch.cat([s.contiguous().reshape(-1) for s in samples])
+    offsets, geoms, off = [], [], 0
+    for s, a in zip(samples, img_aug):
+        H, W = int(s.shape[1]), int(s.shape[2])
+        for (rW, rH), crop in zip(a["resize_dims"], a["crop"]):
+            offsets.append(off)
+            geoms.append((H, W, int(rW), int(rH), int(crop[0]), int(crop[1])))
+            off += H * W * 3
+    out = ops.prepare_images(flat, offsets, geoms, size, norm["mean"], norm["std"], norm["to_rgb"])
+    return out.view(len(samples), N, 3, *size)

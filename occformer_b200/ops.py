@@ -971,3 +971,48 @@ def lidarseg_occupancy(pts, counts, pc_range, grid, panoptic, empty_id, ignore):
     _call("occ_lidarseg_occupancy", pts, ld, (ctypes.c_longlong * (B + 1))(*offsets), B, *r, X, Y, Z, int(panoptic),
           int(empty_id), int(ignore), invalid, ws, ws.numel(), out)
     return out, invalid
+
+
+# ----------------------------------------------------------------------------------------------- camera images
+_prep_tables = {}  # (device, source size, resized size) -> int32 resample table of one axis (image_prep.resample_table)
+_prep_norms = {}   # (device, mean, std, to_rgb) -> float32 (3, 256) normalisation table
+_prep_ws = {}      # (device, stream) -> grow-only uint8 workspace of occ_prepare_images
+
+
+def _prep_table(dev, in_size, out_size):
+    key = (str(dev), in_size, out_size)
+    t = _prep_tables.get(key)
+    if t is None:
+        from .image_prep import resample_table
+        t = torch.from_numpy(resample_table(in_size, out_size)).to(dev)
+        _prep_tables[key] = t
+    return t
+
+
+def prepare_images(frames, offsets, geoms, input_size, mean, std, to_rgb):
+    """M camera images from uint8 BGR frames (occ_prepare_images): frames a flat uint8 CUDA buffer, image m the H x W x 3
+    bytes at offsets[m], geoms[m] = (H, W, rW, rH, x0, y0) -> float32 (M, 3, fH, fW).  The coefficient and normalisation
+    tables are built once per geometry and config and kept on the device; no synchronisation."""
+    M = len(geoms)
+    fH, fW = (int(v) for v in input_size)
+    dev = frames.device
+    geom = (ctypes.c_int * (6 * M))(*[int(v) for g in geoms for v in g])
+    nkey = (str(dev), tuple(mean), tuple(std), bool(to_rgb))
+    norm = _prep_norms.get(nkey)
+    if norm is None:
+        from .image_prep import normalize_table
+        norm = torch.from_numpy(normalize_table(mean, std, to_rgb)).to(dev)
+        _prep_norms[nkey] = norm
+    tables = []
+    for H, W, rW, rH, _, _ in geoms:
+        tables += [_prep_table(dev, W, rW).data_ptr(), _prep_table(dev, H, rH).data_ptr()]
+    nbytes = lib().occ_prepare_images_workspace_bytes(geom, M, fH, fW)
+    key = (str(dev), torch.cuda.current_stream(dev).cuda_stream)
+    ws = _prep_ws.get(key)
+    if ws is None or ws.numel() < max(nbytes, 16):
+        ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
+        _prep_ws[key] = ws
+    out = torch.empty((M, 3, fH, fW), dtype=torch.float32, device=dev)
+    _call("occ_prepare_images", frames, frames.numel(), (ctypes.c_longlong * M)(*offsets), geom, M, fH, fW,
+          (ctypes.c_longlong * (2 * M))(*tables), norm, int(bool(to_rgb)), ws, ws.numel(), out)
+    return out

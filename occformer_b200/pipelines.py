@@ -1,4 +1,5 @@
-"""Loader transforms that leave the occupancy ground truth to the GPU (occformer_b200.targets).
+"""Loader transforms that leave the occupancy ground truth (occformer_b200.targets) or the camera images' resize, crop and
+normalisation (occformer_b200.image_prep, the LoadMultiViewImageFrames_* transforms at the end of this file) to the GPU.
 
     LoadNuscOccupancyPoints          = LoadNuscOccupancyAnnotations          P/datasets/pipelines/loading_nusc_occ.py:13-120
     LoadNuscPanopticOccupancyPoints  = LoadNuscPanopticOccupancyAnnotations  P/datasets/pipelines/loading_nusc_panoptic_occ.py:32-145
@@ -109,3 +110,121 @@ class LoadNuscPanopticOccupancyPoints(_OccupancyPoints):
             sem[hit] = mapped
             pan[hit] = mapped * 1e3 + (pan[hit] - label * 1e3)
         return pan.reshape(-1, 1)
+
+
+# ---------------------------------------------------------------------------------------------- camera images
+class _ImageFrames:
+    """the shared part of the two image transforms: test-mode sample_augmentation (loading_nusc_imgs.py:84-95), the
+    post-homography in the reference's float32 torch arithmetic (:39-53), and the frame decode"""
+
+    def __init__(self, data_config, is_train=False, img_norm_cfg=None):
+        if is_train:
+            raise ValueError(f"{type(self).__name__}: is_train=True is not supported: the package has no training step, "
+                             "and CreateDepthFromLiDAR reads the image size from the normalised images; keep the "
+                             "reference transform for training pipelines")
+        from .image_prep import norm_config
+        self.is_train, self.data_config, self.img_norm_cfg = is_train, data_config, img_norm_cfg
+        self.norm = norm_config(img_norm_cfg)
+
+    def sample_augmentation(self, H, W):
+        fH, fW = self.data_config["input_size"]
+        resize = float(fW) / float(W)
+        resize += self.data_config.get("resize_test", 0.0)
+        resize_dims = (int(W * resize), int(H * resize))
+        newW, newH = resize_dims
+        crop_h = int((1 - np.mean(self.data_config["crop_h"])) * newH) - fH
+        crop_w = int(max(0, newW - fW) / 2)
+        return resize, resize_dims, (crop_w, crop_h, crop_w + fW, crop_h + fH)
+
+    @staticmethod
+    def post_homography(resize, crop):
+        """(post_rot (3, 3), post_tran (3,)) of img_transform with flip False and rotate 0"""
+        post_rot2 = torch.eye(2) * resize
+        post_tran2 = torch.zeros(2) - torch.Tensor(crop[:2])
+        A = torch.Tensor([[np.cos(0.0), np.sin(0.0)], [-np.sin(0.0), np.cos(0.0)]])
+        b = torch.Tensor([crop[2] - crop[0], crop[3] - crop[1]]) / 2
+        b = A.matmul(-b) + b
+        post_rot2 = A.matmul(post_rot2)
+        post_tran2 = A.matmul(post_tran2) + b
+        post_rot, post_tran = torch.eye(3), torch.zeros(3)
+        post_rot[:2, :2] = post_rot2
+        post_tran[:2] = post_tran2
+        return post_rot, post_tran
+
+    @staticmethod
+    def decode(path):
+        """cv2.imread(path, IMREAD_UNCHANGED): the pixels of mmcv.imread(path, 'unchanged') with its cv2 backend"""
+        import cv2
+        img = cv2.imread(path, cv2.IMREAD_UNCHANGED)
+        if img is None:
+            raise FileNotFoundError(path)
+        if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != 3:
+            raise ValueError(f"{path}: a 3-channel uint8 frame is needed, got {img.dtype} {img.shape}")
+        return img
+
+    def camera(self, img):
+        """one decoded frame -> (resize_dims, crop, post_rot, post_tran)"""
+        resize, resize_dims, crop = self.sample_augmentation(img.shape[0], img.shape[1])
+        return (resize_dims, crop) + self.post_homography(resize, crop)
+
+    def img_aug(self, dims, crops):
+        return dict(resize_dims=[list(d) for d in dims], crop=[list(c) for c in crops],
+                    input_size=list(self.data_config["input_size"]), **self.norm)
+
+
+@PIPELINES.register_module()
+class LoadMultiViewImageFrames_OccFormer(_ImageFrames):
+    """LoadMultiViewImageFromFiles_OccFormer (loading_nusc_imgs.py:10-179) in test mode, leaving the resize, crop and
+    normalisation to the GPU (image_prep.prepare_images, called by OccupancyFormer.extract_img_feat).  img_inputs[0] is
+    the decoded uint8 (N, H, W, 3) BGR frames; img_inputs[1:] are the reference's; results['img_aug'] describes each
+    camera's resize and crop and the normalisation, and must be collected into the img_metas (Collect3D meta_keys).
+    results['canvas'] (the cropped uint8 images, read only by a commented-out visualisation) is not produced."""
+
+    def __call__(self, results):
+        cam_names = self.data_config["cams"]
+        results["cam_names"] = cam_names
+        frames, rots, trans, intrins, post_rots, post_trans, sensor2sensors, dims, crops = ([] for _ in range(9))
+        for cam_name in cam_names:
+            cam_data = results["curr"]["cams"][cam_name]
+            img = self.decode(cam_data["data_path"])
+            intrin = torch.Tensor(cam_data["cam_intrinsic"])
+            sensor2lidar = torch.tensor(results["lidar2cam_dic"][cam_name]).inverse().float()
+            resize_dims, crop, post_rot, post_tran = self.camera(img)
+            frames.append(torch.from_numpy(img))
+            intrins.append(intrin)
+            rots.append(sensor2lidar[:3, :3])
+            trans.append(sensor2lidar[:3, 3])
+            post_rots.append(post_rot)
+            post_trans.append(post_tran)
+            sensor2sensors.append(sensor2lidar)
+            dims.append(resize_dims)
+            crops.append(crop)
+        if len({tuple(f.shape) for f in frames}) != 1:
+            raise ValueError("LoadMultiViewImageFrames_OccFormer: the cameras of a sample need one frame size")
+        gt_depths = [torch.zeros(1) for _ in cam_names]
+        results["img_inputs"] = tuple(torch.stack(x) for x in (frames, rots, trans, intrins, post_rots, post_trans,
+                                                                gt_depths, sensor2sensors))
+        results["img_aug"] = self.img_aug(dims, crops)
+        return results
+
+
+@PIPELINES.register_module()
+class LoadMultiViewImageFrames_SemanticKitti(_ImageFrames):
+    """LoadMultiViewImageFromFiles_SemanticKitti (loading_kitti_imgs.py:12-146) in test mode, leaving the resize, crop
+    and normalisation to the GPU: img_inputs[0] is the decoded uint8 (1, H, W, 3) BGR frame, img_inputs[1:] are the
+    reference's, results['raw_img'] is kept and results['img_aug'] added; results['canvas'] is not produced."""
+
+    def __call__(self, results):
+        img_filenames = results["img_filename"]
+        assert len(img_filenames) == 1
+        img = self.decode(img_filenames[0])
+        results["raw_img"] = img
+        resize_dims, crop, post_rot, post_tran = self.camera(img)
+        intrin = torch.Tensor(results["cam_intrinsic"][0])
+        lidar2cam = torch.Tensor(results["lidar2cam"][0])
+        cam2lidar = lidar2cam.inverse()
+        res = [torch.from_numpy(img), cam2lidar[:3, :3], cam2lidar[:3, 3], intrin, post_rot, post_tran, torch.zeros(1),
+               cam2lidar]
+        results["img_inputs"] = tuple(x[None] for x in res)
+        results["img_aug"] = self.img_aug([resize_dims], [crop])
+        return results
