@@ -295,6 +295,11 @@ __global__ void vp_nchw_to_nhwc_kernel(const float* __restrict__ in, int C, int 
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// Launch grid sizes in 64-bit: n + per - 1 overflows int within per of the 2^31 limit the entry points allow.
+static unsigned blocks_for(long long n, long long per) { return (unsigned)((n + per - 1) / per); }
+// vp_pool_kernel: one warp per 32 voxels, 8 warps per block
+static unsigned pool_blocks(int V) { return blocks_for(blocks_for(V, 32), 8); }
+
 struct VpWorkspace {
   int *head, *counts, *next, *vox_id;  // head and counts are adjacent: one memset clears both
 };
@@ -340,11 +345,10 @@ extern "C" int occ_lift_splat(const float* depth_prob, const float* feat_cl, con
   // head[V] and counts[V] are adjacent in the workspace: one memset
   OCC_MEMSET(ws.head, 0, reinterpret_cast<char*>(ws.counts + V) - reinterpret_cast<char*>(ws.head), stream);
   const VpGrid vg{dx0, dx1, dx2, bx0, bx1, bx2, nx0, nx1, nx2, X, Y, Z};
-  vp_index_geom_kernel<<<(P + 255) / 256, 256, 0, stream>>>(geom, P, N * D * HW, vg, ws.vox_id, ws.counts, ws.head, ws.next);
+  vp_index_geom_kernel<<<blocks_for(P, 256), 256, 0, stream>>>(geom, P, N * D * HW, vg, ws.vox_id, ws.counts, ws.head, ws.next);
   OCC_LAUNCH_CHECK();
-  vp_pool_kernel<0><<<((V + 31) / 32 + 7) / 8, 256, 0, stream>>>(ws.head, ws.next, V, C, depth_prob, feat_cl,
-                                                                 make_fastdiv((uint32_t)D * HW), make_fastdiv(HW), out,
-                                                                 out_split);
+  vp_pool_kernel<0><<<pool_blocks(V), 256, 0, stream>>>(ws.head, ws.next, V, C, depth_prob, feat_cl,
+                                                        make_fastdiv((uint32_t)D * HW), make_fastdiv(HW), out, out_split);
   OCC_LAUNCH_CHECK();
   return OCC_OK;
 }
@@ -363,12 +367,12 @@ extern "C" int occ_bev_pool(const float* feats, const long long* coords, float* 
   OCC_REQUIRE(vp_layout(workspace, n, V, &ws) <= workspace_bytes);
   OCC_MEMSET(ws.head, 0, reinterpret_cast<char*>(ws.counts + V) - reinterpret_cast<char*>(ws.head), stream);
   if (n > 0) {
-    vp_index_coords_kernel<<<(n + 255) / 256, 256, 0, stream>>>(coords, n, B, X, Y, Z, ws.vox_id, ws.counts, ws.head,
-                                                                ws.next);
+    vp_index_coords_kernel<<<blocks_for(n, 256), 256, 0, stream>>>(coords, n, B, X, Y, Z, ws.vox_id, ws.counts, ws.head,
+                                                                  ws.next);
     OCC_LAUNCH_CHECK();
   }
-  vp_pool_kernel<1><<<((V + 31) / 32 + 7) / 8, 256, 0, stream>>>(ws.head, ws.next, V, C, nullptr, feats, make_fastdiv(1),
-                                                                 make_fastdiv(1), out, nullptr);
+  vp_pool_kernel<1><<<pool_blocks(V), 256, 0, stream>>>(ws.head, ws.next, V, C, nullptr, feats, make_fastdiv(1),
+                                                        make_fastdiv(1), out, nullptr);
   OCC_LAUNCH_CHECK();
   return OCC_OK;
 }
@@ -377,9 +381,9 @@ extern "C" int occ_bev_pool(const float* feats, const long long* coords, float* 
 extern "C" int occ_lift_prologue(const float* depth_logits, const float* img_feat, float* depth_prob,
                                  float* feat_cl, int BN, int D, int C, int HW, cudaStream_t stream) {
   OCC_REQUIRE(depth_logits && img_feat && depth_prob && feat_cl && BN > 0 && D > 0 && C > 0 && HW > 0);
-  vp_depth_softmax_kernel<<<(BN * HW + 127) / 128, 128, 0, stream>>>(depth_logits, BN, D, HW, depth_prob);
+  vp_depth_softmax_kernel<<<blocks_for((long long)BN * HW, 128), 128, 0, stream>>>(depth_logits, BN, D, HW, depth_prob);
   OCC_LAUNCH_CHECK();
-  dim3 grid((HW + 31) / 32, (C + 31) / 32, BN), block(32, 8);
+  dim3 grid(blocks_for(HW, 32), blocks_for(C, 32), BN), block(32, 8);
   vp_nchw_to_nhwc_kernel<<<grid, block, 0, stream>>>(img_feat, C, HW, feat_cl);
   OCC_LAUNCH_CHECK();
   return OCC_OK;
@@ -413,11 +417,11 @@ extern "C" int occ_voxel_pool_geom(const float* feats, const float* geom, float*
   OCC_REQUIRE(vp_layout(workspace, P, V, &ws) <= workspace_bytes);
   OCC_MEMSET(ws.head, 0, reinterpret_cast<char*>(ws.counts + V) - reinterpret_cast<char*>(ws.head), stream);
   const VpGrid vg{dx0, dx1, dx2, bx0, bx1, bx2, nx0, nx1, nx2, X, Y, Z};
-  vp_index_geom_kernel<<<(P + 255) / 256, 256, 0, stream>>>(geom, P, points_per_batch, vg, ws.vox_id, ws.counts, ws.head,
-                                                             ws.next);
+  vp_index_geom_kernel<<<blocks_for(P, 256), 256, 0, stream>>>(geom, P, points_per_batch, vg, ws.vox_id, ws.counts,
+                                                                ws.head, ws.next);
   OCC_LAUNCH_CHECK();
-  vp_pool_kernel<1><<<((V + 31) / 32 + 7) / 8, 256, 0, stream>>>(ws.head, ws.next, V, C, nullptr, feats, make_fastdiv(1),
-                                                                 make_fastdiv(1), out, nullptr);
+  vp_pool_kernel<1><<<pool_blocks(V), 256, 0, stream>>>(ws.head, ws.next, V, C, nullptr, feats, make_fastdiv(1),
+                                                        make_fastdiv(1), out, nullptr);
   OCC_LAUNCH_CHECK();
   return OCC_OK;
 }
@@ -605,7 +609,7 @@ extern "C" int occ_lss_geometry(const float* frustum, int P, const float* rots, 
   OCC_REQUIRE(P > 0 && B > 0 && N > 0 && (intrin_cols == 3 || intrin_cols == 4) && (bda_dim == 3 || bda_dim == 4));
   OCC_REQUIRE(intrin_rows >= 3 && intrin_rows <= 4 && intrin_rows <= intrin_cols + 1);
   OCC_REQUIRE((long long)B * N <= 65535);
-  dim3 grid((P + 255) / 256, B * N);
+  dim3 grid(blocks_for(P, 256), B * N);
   occ::lss_geometry_kernel<<<grid, 256, 0, stream>>>(frustum, P, rots, trans, intrins, intrin_rows, intrin_cols, post_rots,
                                                      post_trans,
                                                      bda, bda_dim, N, geom);
@@ -644,7 +648,7 @@ extern "C" int occ_lift_splat_fused(const float* depth_logits, long long logits_
   OCC_REQUIRE(vp_layout(workspace, P, V, &ws) <= workspace_bytes);
   OCC_MEMSET(ws.head, 0, reinterpret_cast<char*>(ws.counts + V) - reinterpret_cast<char*>(ws.head), stream);
   const VpGrid vg{dx0, dx1, dx2, bx0, bx1, bx2, nx0, nx1, nx2, X, Y, Z};
-  const int tiles_p = (HW + 31) / 32, tiles_c = (C + 31) / 32;
+  const int tiles_p = (int)blocks_for(HW, 32), tiles_c = (int)blocks_for(C, 32);
   const int nb_front = B * N * tiles_p;
   const long long nb = (long long)nb_front + (long long)B * N * tiles_p * tiles_c;
   OCC_REQUIRE(nb < (1ll << 31));
@@ -654,9 +658,8 @@ extern "C" int occ_lift_splat_fused(const float* depth_logits, long long logits_
                                                       depth_prob, feat_cl, ws.vox_id, ws.counts, ws.head, ws.next, nb_front,
                                                       tiles_p, tiles_c);
   OCC_LAUNCH_CHECK();
-  vp_pool_kernel<0><<<((V + 31) / 32 + 7) / 8, 256, 0, stream>>>(ws.head, ws.next, V, C, depth_prob, feat_cl,
-                                                                 make_fastdiv((uint32_t)D * HW), make_fastdiv(HW), out,
-                                                                 out_split);
+  vp_pool_kernel<0><<<pool_blocks(V), 256, 0, stream>>>(ws.head, ws.next, V, C, depth_prob, feat_cl,
+                                                        make_fastdiv((uint32_t)D * HW), make_fastdiv(HW), out, out_split);
   OCC_LAUNCH_CHECK();
   return OCC_OK;
 }

@@ -161,7 +161,11 @@ class VoxelPoolWorkspace:
         return self._ints(self.off_vox_id, self.P)
 
 
-_ws_cache = {}  # (B, X, Y, Z, device) -> (uint8 buffer, point capacity): one grow-only buffer per grid
+# (B, X, Y, Z, device) -> (uint8 buffer, point capacity, superseded buffers): one grow-only buffer per grid.  A CUDA
+# graph captured before the buffer grew still points at the buffer it was captured with, so the superseded ones stay
+# referenced.  Point capacities double, so the point arrays of all the superseded buffers together are no larger than
+# the newest one's.
+_ws_cache = {}
 
 
 def _workspace(n_points, B, X, Y, Z, device):
@@ -171,7 +175,8 @@ def _workspace(n_points, B, X, Y, Z, device):
     if ent is None or ent[1] < n_points:
         cap = 1 << (n_points - 1).bit_length()  # next power of two: the drop-in bev_pool sees a different n every sample
         nbytes = lib().occ_voxel_pool_workspace_bytes(cap, B, X, Y, Z)
-        ent = (torch.zeros(nbytes, dtype=torch.uint8, device=device), cap)
+        old = [] if ent is None else ent[2] + [ent[0]]
+        ent = (torch.zeros(nbytes, dtype=torch.uint8, device=device), cap, old)
         _ws_cache[key] = ent
     return VoxelPoolWorkspace(ent[0], n_points, B, X, Y, Z)
 

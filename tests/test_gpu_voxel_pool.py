@@ -5,6 +5,8 @@ import numpy as np
 import pytest
 import torch
 
+import lift_ref
+from lift_ref import check_bookkeeping
 from oracle import port
 from occformer_b200 import synth
 from occformer_b200.common import twin_of
@@ -21,41 +23,6 @@ def _setup(grid_name, cams, input_size, B, N, C, seed):
     D, fH, fW = frustum.shape[:3]
     dd, feat = synth.lift_inputs(B, N, D, fH, fW, C, seed=seed)
     return gc, geom, dx, bx, nx, dd, feat
-
-
-def _check_bookkeeping(ws, gf, kept, B, X, Y, Z):
-    """vox_id / kept mask / per-voxel counts must equal the reference's index math exactly."""
-    vox = ws.vox_id.cpu().long()
-    ref_lin = ((gf[:, 3] * X + gf[:, 0]) * Y + gf[:, 1]) * Z + gf[:, 2]
-    ref_vox = torch.where(kept, ref_lin, torch.full_like(ref_lin, -1))
-    assert torch.equal(vox, ref_vox), f"voxel ids differ at {(vox != ref_vox).sum()} points"
-    counts = ws.counts.cpu().long()
-    ref_counts = torch.bincount(ref_lin[kept], minlength=B * X * Y * Z)
-    assert torch.equal(counts, ref_counts)
-    assert int(counts.sum()) == int(kept.sum())
-    # interval bookkeeping in the reference's own rank order (bev_pool.py:86-93 / QuickCumsumCuda :40-45)
-    uniq, lens = port.bev_pool_bookkeeping(gf[kept], B, Z, X, Y)
-    nzv = torch.nonzero(counts).flatten()
-    b = nzv // (X * Y * Z); r = nzv % (X * Y * Z); x = r // (Y * Z); y = (r // Z) % Y; z = r % Z
-    my_ranks = x * (Y * Z * B) + y * (Z * B) + z * B + b
-    order = my_ranks.argsort()
-    assert torch.equal(my_ranks[order], uniq) and torch.equal(counts[nzv][order], lens)
-    # per-voxel point lists: walking head/next visits every kept point exactly once, inside its own voxel
-    head, nxt = ws.head.cpu().long(), ws.next.cpu().long()
-    assert torch.equal(head != 0, counts != 0)
-    visited = torch.zeros(vox.numel(), dtype=torch.long)
-    cur = head.clone()
-    vidx = torch.arange(head.numel())
-    for _ in range(int(counts.max()) + 1):
-        live = cur != 0
-        if not bool(live.any()):
-            break
-        p = cur[live] - 1
-        assert torch.equal(vox[p], vidx[live]), "a list contains a point of another voxel"
-        visited[p] += 1
-        cur = torch.where(live, torch.cat([nxt, torch.zeros(1, dtype=torch.long)])[(cur - 1).clamp(min=-1)], cur)
-    assert not bool((cur != 0).any()), "a list is longer than its voxel's count"
-    assert torch.equal(visited, kept.long()), "kept points and list membership differ"
 
 
 @pytest.mark.parametrize("B", [1, 2])
@@ -81,7 +48,7 @@ def test_lift_splat_pr1(cuda, B):
     X, Y, Z = vt.grid_size()
     ws = ops._workspace(geom.numel() // 3, B, X, Y, Z, cuda)
     torch.cuda.synchronize()
-    _check_bookkeeping(ws, gf, kept, B, X, Y, Z)
+    check_bookkeeping(ws, gf, kept, B, X, Y, Z)
     if B == 2:  # golden fixture generated from the REAL reference (oracle/gen_golden.py)
         gd = golden("voxel_pool_pr1.npz")
         assert np.array_equal(gd["geom"], geom.numpy())
@@ -130,7 +97,7 @@ def test_lift_splat_nusc_properties(cuda):
     X, Y, Z = vt.grid_size()
     ws = ops._workspace(idx.shape[0], B, X, Y, Z, cuda)
     torch.cuda.synchronize()
-    _check_bookkeeping(ws, gf, kept, B, X, Y, Z)
+    check_bookkeeping(ws, gf, kept, B, X, Y, Z)
     # mass conservation per channel: sum_v out[v,c] == sum_{kept p} depth[p] * feat[pix(p), c]
     prob_ref = dd.softmax(1)
     D, HW = prob_ref.shape[1], prob_ref.shape[2] * prob_ref.shape[3]
@@ -161,7 +128,7 @@ def test_lift_splat_other_workloads(cuda, wl):
     X, Y, Z = vt.grid_size()
     ws = ops._workspace(idx.shape[0], B, X, Y, Z, cuda)
     torch.cuda.synchronize()
-    _check_bookkeeping(ws, gf, kept, B, X, Y, Z)
+    check_bookkeeping(ws, gf, kept, B, X, Y, Z)
     prob_ref = dd.softmax(1)
     D, HW = prob_ref.shape[1], prob_ref.shape[2] * prob_ref.shape[3]
     wsum = (prob_ref.reshape(N, D, HW) * kept.view(N, D, HW)).sum(1)
@@ -225,7 +192,8 @@ class _PassThrough(torch.nn.Module):
 def test_forward_fused_front_end_vs_oracle(cuda, wl, B):
     """ViewTransformerLiftSplatShootVoxel.forward(input) = one fused front kernel (depth softmax + get_geometry + voxel
     index + lists + NHWC transpose) + the pooling kernel, fed with channel slices of the (B*N, D+C, fH, fW) map (no copies):
-    same voxel bookkeeping as the oracle's index math on the oracle geometry, same sums, same depth_prob."""
+    same voxel bookkeeping as the oracle's index math on the oracle geometry away from cell boundaries, the grid within
+    lift_ref's bound of fp64 pooling over the kernel's own voxel ids, same depth_prob."""
     from occformer_b200 import ops
     from occformer_b200.view_transformer import ViewTransformerLiftSplatShootVoxel
     C = 32
@@ -255,8 +223,27 @@ def test_forward_fused_front_end_vs_oracle(cuda, wl, B):
     frac = ((geom.view(-1, 3) - (bx - dx / 2.0)) / dx)
     near = ((frac - frac.round()).abs() < 1e-4).any(-1)
     assert bool((~flips | near).all()), "index flips away from cell boundaries"
-    if int(flips.sum()) == 0:
-        assert_close(voxel, ref, 1e-4, f"{wl} forward pooled grid")  # fp32 exp + summation-order noise on near-cancelling sums
-        assert torch.equal(ops.to_split(voxel.permute(0, 2, 3, 4, 1).contiguous()).view(torch.int32),
-                           twin_of(voxel).view(torch.int32))
+    # the grid and its twin in every case: fp64 pooling over the kernel's own voxel ids (lift_ref.assert_pooled)
+    feat_cl = feat.permute(0, 2, 3, 1).reshape(-1, C).to(cuda)
+    lift_ref.assert_pooled(voxel.permute(0, 2, 3, 4, 1).reshape(-1, C), ws.vox_id.long(), prob,
+                           lift_ref.lift_rows(B, N, D, fH * fW), feat_cl, B * X * Y * Z, f"{wl} forward pooled grid")
+    assert torch.equal(ops.to_split(voxel.permute(0, 2, 3, 4, 1).contiguous()).view(torch.int32),
+                       twin_of(voxel).view(torch.int32))
     print(f"{wl}: forward front-end flips {int(flips.sum())} of {flips.numel()}")
+
+
+def test_workspace_growth_keeps_superseded_buffers_alive(cuda):
+    """a grid's pooling workspace grows when a call brings more points; a CUDA graph captured before still points at the
+    old buffer, so the cache keeps it referenced"""
+    import gc
+    import weakref
+    from occformer_b200 import ops
+    key = (1, 3, 5, 7)
+    ent = ops._ws_cache.get((*key, str(cuda)))
+    n = 2 * (ent[1] if ent else 64)
+    small = ops._workspace(n, *key, cuda).buf
+    old = weakref.ref(small)
+    del small
+    big = ops._workspace(4 * n, *key, cuda).buf
+    gc.collect()
+    assert old() is not None and old().data_ptr() != big.data_ptr(), "the superseded workspace was freed"
