@@ -517,6 +517,42 @@ int occ_prepare_images(const unsigned char* frames, long long frame_bytes, const
                        const int* geom /*HOST*/, int M, int fH, int fW, const long long* tables /*HOST*/,
                        const float* norm, int swap_rb, void* ws, size_t ws_bytes, float* out, occ_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * Camera frames from their JPEG files (csrc/jpeg_decode.cu): step 1 of the test loaders' image side,
+ *   LoadMultiViewImageFromFiles_OccFormer     P/datasets/pipelines/loading_nusc_imgs.py:181-195 (mmcv.imread, cv2)
+ * bit for bit as cv2.imdecode(buf, IMREAD_UNCHANGED) with libjpeg-turbo: Huffman-coded sequential DCT, 8-bit samples,
+ * three components (YCbCr) in one interleaved scan, luma sampling 1x1 / 2x1 / 2x2 with chroma 1x1, any restart interval;
+ * libjpeg's islow IDCT with the output + 128 clamped to [0, 255] (libjpeg-turbo's SIMD IDCT, not its wrapping C table),
+ * fancy (triangle) chroma upsampling with edges replicated at the component's real size, libjpeg's YCbCr -> RGB tables.
+ * occformer_b200/jpeg.py parses the headers and refuses everything else on the host.
+ *   data         uint8, data_bytes bytes, holding the files
+ *   scan         HOST int64 (M, 2): byte offset in data and length of image m's entropy-coded segment (from the end of
+ *                the SOS header to the EOI marker); offset + length <= data_bytes, length < 2^28
+ *   geom         HOST int32 (M, 5): H, W (1..16384), luma sampling hs, vs ((1,1), (2,1) or (2,2)), restart interval in
+ *                MCUs (0: none, up to 65535)
+ *   tables       HOST int64 (M, 9): device addresses (4-byte aligned) of the quantisation tables of components 0..2
+ *                (64 int32, natural order; used as 16-bit multipliers, as libjpeg does), their DC Huffman tables and
+ *                their AC Huffman tables (occformer_b200.jpeg.huff_table's flat int32 form)
+ *   out_offsets  HOST int64 (M): byte offset of image m's (H, W, 3) uint8 B, G, R frame in out (out_bytes bytes); only
+ *                those bytes of out are written
+ *   seq_bits     S, 32 .. 2^20: bits per subsequence of the parallel Huffman decode; sync_rounds R, 0 .. 64:
+ *                self-synchronisation rounds before the serial fix-up.  Neither changes the result.
+ *   status       (M, 2) int32, overwritten: status[m, 0] = 0 for a decoded image, else the OR of 1 (a marker other than
+ *                RSTn inside the segment), 2 (RSTn markers missing, surplus or out of order), 4 (an invalid Huffman
+ *                code or a coefficient run past 63), 8 (the data of a restart interval, or of the scan, ends before
+ *                its last MCU); status[m, 1] = subsequences the fix-up decoded again serially.  libjpeg would warn and
+ *                fill in grey instead of failing; the frame of a failed image is undefined, but nothing is written
+ *                outside it.
+ *   ws           occ_decode_jpeg_workspace_bytes(scan, geom, M, seq_bits) bytes, 16-byte aligned
+ * 1 <= M <= 96.  11 + R enqueued launches and memsets per call whatever M and the data, no host synchronisation
+ * (capturable in a CUDA graph).  Returns -1 for a bad M, S, R, geometry, segment, table address, output range or a
+ * short or misaligned workspace, with nothing enqueued. */
+size_t occ_decode_jpeg_workspace_bytes(const long long* scan /*HOST*/, const int* geom /*HOST*/, int M, int seq_bits);
+int occ_decode_jpeg(const unsigned char* data, long long data_bytes, const long long* scan /*HOST*/,
+                    const int* geom /*HOST*/, const long long* tables /*HOST*/, const long long* out_offsets /*HOST*/,
+                    int M, int seq_bits, int sync_rounds, void* ws, size_t ws_bytes, unsigned char* out,
+                    long long out_bytes, int* status, occ_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -116,8 +116,17 @@ class OccupancyFormer(nn.Module):
         The reference clones the image features for a head that ignores them; they are handed on as they are.
         imgs may also be the uint8 (B, N, H, W, 3) BGR frames of occformer_b200.pipelines' LoadMultiViewImageFrames_*
         transforms: they are resized, cropped and normalised on the GPU first (image_prep.prepare_images), from the
-        'img_aug' of each sample's metas."""
+        'img_aug' of each sample's metas.  An empty uint8 (B, N, 0) imgs is LoadMultiViewJpegBytes_OccFormer's
+        placeholder: the JPEG files in each 'img_aug' are decoded on the GPU first (image_prep.decode_jpeg)."""
         imgs = img[0]
+        if torch.is_tensor(imgs) and imgs.dtype == torch.uint8 and imgs.dim() == 3 and imgs.shape[-1] == 0:
+            if img_metas is None or any("jpeg" not in m.get("img_aug", {}) for m in img_metas):
+                raise ValueError("OccupancyFormer: the empty image placeholder needs each sample's 'img_aug' meta with "
+                                 "its 'jpeg' files, which LoadMultiViewJpegBytes_OccFormer produces; add 'img_aug' to "
+                                 "Collect3D's meta_keys")
+            augs = [m["img_aug"] for m in img_metas]
+            names = [a.get("jpeg_files") for a in augs]
+            imgs = image_prep.decode_jpeg([a["jpeg"] for a in augs], None if None in names else names)
         if (imgs.dtype if torch.is_tensor(imgs) else imgs[0].dtype) == torch.uint8:
             if img_metas is None or any("img_aug" not in m for m in img_metas):
                 raise ValueError("OccupancyFormer: uint8 camera frames need each sample's 'img_aug' meta, which the "

@@ -7,6 +7,10 @@ The loader transforms of occformer_b200.pipelines hand the model uint8 BGR frame
     {"resize_dims": [[rW, rH], ...], "crop": [[x0, y0, x1, y1], ...],   # one per camera, as sample_augmentation gives
      "input_size": [fH, fW], "mean": [3 floats], "std": [3 floats], "to_rgb": bool}   # mmlabNormalize's config
 
+decode_jpeg decodes the camera files themselves on the device (csrc/jpeg_decode.cu), bit for bit as cv2.imdecode,
+into the frames prepare_images takes; the loader then ships the JPEG bytes instead of the decoded frames
+(pipelines.LoadMultiViewJpegBytes_OccFormer).
+
 The host part here is table building: Pillow's bicubic coefficients per (source size, resized size) of an axis and the
 normalisation as a 3 x 256 table, both in float64 numpy, one operation at a time as x86-64 builds of Pillow and OpenCV
 compute them (no fused multiply-add).  ops.prepare_images caches them on the device.
@@ -16,7 +20,7 @@ import math
 import numpy as np
 import torch
 
-from . import ops
+from . import jpeg, ops
 
 PRECISION_BITS = 22  # Pillow's resample.c: 32 - 8 - 2
 DEFAULT_NORM = dict(mean=[123.675, 116.28, 103.53], std=[58.395, 57.12, 57.375], to_rgb=True)  # mmlabNormalize's
@@ -116,3 +120,55 @@ def prepare_images(frames, img_aug):
             off += H * W * 3
     out = ops.prepare_images(flat, offsets, geoms, size, norm["mean"], norm["std"], norm["to_rgb"])
     return out.view(len(samples), N, 3, *size)
+
+
+def decode_jpeg(files, names=None, seq_bits=ops.JPEG_SEQ_BITS, sync_rounds=ops.JPEG_SYNC_ROUNDS):
+    """files: B samples, each a list of N JPEG files (bytes-like) -> uint8 CUDA (B, N, H, W, 3) B, G, R frames when all
+    share one size, else a list of B per-sample (N, H_i, W_i, 3) tensors: the two forms prepare_images takes, equal to
+    cv2.imdecode(buf, IMREAD_UNCHANGED) of each file.  The files travel in one pinned host buffer and one host-to-device
+    copy, and decode in one occ_decode_jpeg call; one status read-back then raises ValueError naming a file whose
+    entropy-coded data is corrupt (libjpeg would warn and fill in grey).  names: the same nesting of file names for the
+    messages (default: sample and camera indices).  seq_bits / sync_rounds tune the parallel Huffman decode and do not
+    change the result."""
+    samples = [list(s) for s in files]
+    if not samples or any(not s for s in samples):
+        raise ValueError("decode_jpeg: needs at least one sample of at least one file")
+    label = [[names[b][n] if names is not None else f"sample {b} camera {n}" for n in range(len(s))]
+             for b, s in enumerate(samples)]
+    headers, flat = [], []
+    for s, lab in zip(samples, label):
+        for f, name in zip(s, lab):
+            try:
+                headers.append(jpeg.parse(f))
+            except jpeg.JpegError as e:
+                raise ValueError(f"decode_jpeg: {name}: {e}") from None
+            flat.append(memoryview(f).cast("B"))
+    for s, lab, b0 in zip(samples, label, np.cumsum([0] + [len(s) for s in samples])[:-1]):
+        sizes = {(h.height, h.width) for h in headers[b0:b0 + len(s)]}
+        if len(sizes) != 1:
+            raise ValueError(f"decode_jpeg: the cameras of a sample need one frame size, got {sorted(sizes)}")
+    offsets = np.cumsum([0] + [len(f) for f in flat]).tolist()
+    host = torch.empty(offsets[-1], dtype=torch.uint8, pin_memory=True)
+    hv = host.numpy()
+    for f, o in zip(flat, offsets):
+        hv[o:o + len(f)] = np.frombuffer(f, np.uint8)
+    data = host.to(torch.cuda.current_device(), non_blocking=True)
+    out, status = ops.decode_jpeg(data, offsets[:-1], headers, seq_bits, sync_rounds)
+    bad = status[:, 0].cpu()
+    if bool(bad.any()):
+        m = int(bad.nonzero()[0, 0])
+        b = int(np.searchsorted(np.cumsum([len(s) for s in samples]), m, side="right"))
+        n = m - sum(len(s) for s in samples[:b])
+        raise ValueError(f"decode_jpeg: {label[b][n]}: corrupt entropy-coded data (status {int(bad[m])}: "
+                         + ", ".join(w for bit, w in ((1, "unexpected marker"), (2, "bad restart markers"),
+                                                      (4, "invalid Huffman code or run"), (8, "data ends early"))
+                                     if int(bad[m]) & bit) + ")")
+    shapes = [(len(s), headers[b0].height, headers[b0].width)
+              for s, b0 in zip(samples, np.cumsum([0] + [len(s) for s in samples])[:-1])]
+    if len(set(shapes)) == 1 and len({len(s) for s in samples}) == 1:
+        return out.view(len(samples), *shapes[0], 3)
+    res, o = [], 0
+    for N, H, W in shapes:
+        res.append(out[o:o + N * H * W * 3].view(N, H, W, 3))
+        o += N * H * W * 3
+    return res

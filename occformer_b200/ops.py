@@ -1021,3 +1021,59 @@ def prepare_images(frames, offsets, geoms, input_size, mean, std, to_rgb):
     _call("occ_prepare_images", frames, frames.numel(), (ctypes.c_longlong * M)(*offsets), geom, M, fH, fW,
           (ctypes.c_longlong * (2 * M))(*tables), norm, int(bool(to_rgb)), ws, ws.numel(), out)
     return out
+
+
+# ----------------------------------------------------------------------------------------------- JPEG decoding
+JPEG_SEQ_BITS = 4096    # bits per subsequence of the parallel Huffman decode (scripts/bench_jpeg.py --tune)
+JPEG_SYNC_ROUNDS = 6    # self-synchronisation rounds before the serial fix-up
+JPEG_MAX_IMAGES = 96    # images per occ_decode_jpeg call
+_jpeg_tables = {}       # (device, DQT / DHT bytes) -> int32 table on the device
+_jpeg_ws = {}           # (device, stream) -> (grow-only uint8 workspace of occ_decode_jpeg, superseded workspaces)
+
+
+def _jpeg_table(dev, key, table):
+    k = (str(dev), key)
+    t = _jpeg_tables.get(k)
+    if t is None:
+        t = torch.from_numpy(table).to(dev)
+        _jpeg_tables[k] = t
+    return t
+
+
+def decode_jpeg(data, offsets, headers, seq_bits=JPEG_SEQ_BITS, sync_rounds=JPEG_SYNC_ROUNDS):
+    """M baseline JPEG files -> uint8 B, G, R frames (occ_decode_jpeg): data a flat uint8 CUDA buffer, file m at byte
+    offsets[m], headers[m] = occformer_b200.jpeg.parse of it -> (out: flat uint8 CUDA buffer of the M (H, W, 3) frames
+    back to back, status: int32 CUDA (M, 2), see include/occ_b200.h).  The Huffman and quantisation tables are uploaded
+    once per distinct marker content and kept on the device; no synchronisation."""
+    M = len(headers)
+    if not 1 <= M <= JPEG_MAX_IMAGES:
+        raise ValueError(f"decode_jpeg: 1 to {JPEG_MAX_IMAGES} images per call, got {M}")
+    dev = data.device
+    scan, geom, tables, out_off, total = [], [], [], [], 0
+    for off, h in zip(offsets, headers):
+        scan += [int(off) + h.scan_off, h.scan_len]
+        geom += [h.height, h.width, h.hs, h.vs, h.restart]
+        tables += [_jpeg_table(dev, *q).data_ptr() for q in h.qt]
+        tables += [_jpeg_table(dev, *t).data_ptr() for t in h.dc]
+        tables += [_jpeg_table(dev, *t).data_ptr() for t in h.ac]
+        out_off.append(total)
+        total += h.height * h.width * 3
+    scan = (ctypes.c_longlong * (2 * M))(*scan)
+    geom = (ctypes.c_int * (5 * M))(*geom)
+    nbytes = lib().occ_decode_jpeg_workspace_bytes(scan, geom, M, int(seq_bits))
+    if nbytes == 0:
+        raise RuntimeError(f"occformer_b200: occ_decode_jpeg takes 32 <= seq_bits <= 2^20, got {seq_bits}")
+    key = (str(dev), torch.cuda.current_stream(dev).cuda_stream)
+    ent = _jpeg_ws.get(key)
+    if ent is None or ent[0].numel() < nbytes:
+        # a graph captured before the workspace grew still points at the old one: keep it referenced
+        old = [] if ent is None else ent[1] + [ent[0]]
+        ent = (torch.empty(nbytes, dtype=torch.uint8, device=dev), old)
+        _jpeg_ws[key] = ent
+    ws = ent[0]
+    out = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)
+    status = torch.empty((M, 2), dtype=torch.int32, device=dev)
+    _call("occ_decode_jpeg", data, data.numel(), scan, geom, (ctypes.c_longlong * (9 * M))(*tables),
+          (ctypes.c_longlong * M)(*out_off), M, int(seq_bits), int(sync_rounds), ws, ws.numel(), out, out.numel(),
+          status)
+    return out[:total], status

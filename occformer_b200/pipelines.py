@@ -1,5 +1,6 @@
-"""Loader transforms that leave the occupancy ground truth (occformer_b200.targets) or the camera images' resize, crop and
-normalisation (occformer_b200.image_prep, the LoadMultiViewImageFrames_* transforms at the end of this file) to the GPU.
+"""Loader transforms that leave the occupancy ground truth (occformer_b200.targets), the camera images' resize, crop and
+normalisation (occformer_b200.image_prep, the LoadMultiViewImageFrames_* transforms) or also the JPEG decoding
+(LoadMultiViewJpegBytes_OccFormer, at the end of this file) to the GPU.
 
     LoadNuscOccupancyPoints          = LoadNuscOccupancyAnnotations          P/datasets/pipelines/loading_nusc_occ.py:13-120
     LoadNuscPanopticOccupancyPoints  = LoadNuscPanopticOccupancyAnnotations  P/datasets/pipelines/loading_nusc_panoptic_occ.py:32-145
@@ -227,4 +228,52 @@ class LoadMultiViewImageFrames_SemanticKitti(_ImageFrames):
                cam2lidar]
         results["img_inputs"] = tuple(x[None] for x in res)
         results["img_aug"] = self.img_aug([resize_dims], [crop])
+        return results
+
+
+@PIPELINES.register_module()
+class LoadMultiViewJpegBytes_OccFormer(LoadMultiViewImageFrames_OccFormer):
+    """LoadMultiViewImageFrames_OccFormer without the decode: each camera file's bytes are read and the frame size comes
+    from its SOF header (jpeg.frame_size), so img_aug and img_inputs[1:] are the frame transform's.  results['img_aug']
+    also carries 'jpeg' (the N files' bytes, in camera order) and 'jpeg_files' (their paths); img_inputs[0] is an empty
+    uint8 (N, 0) placeholder, which collates to (B, N, 0), a shape no other transform produces.  OccupancyFormer then
+    decodes the files on the GPU (image_prep.decode_jpeg) and prepares the images from the frames.  Files the device
+    decoder does not take (progressive, grayscale, ...) raise ValueError here, in the loader."""
+
+    def __call__(self, results):
+        from .jpeg import JpegError, frame_size
+        cam_names = self.data_config["cams"]
+        results["cam_names"] = cam_names
+        files, paths, rots, trans, intrins, post_rots, post_trans, sensor2sensors, dims, crops, sizes = (
+            [] for _ in range(11))
+        for cam_name in cam_names:
+            cam_data = results["curr"]["cams"][cam_name]
+            path = cam_data["data_path"]
+            with open(path, "rb") as f:
+                data = f.read()
+            try:
+                H, W = frame_size(data)
+            except JpegError as e:
+                raise ValueError(f"{path}: {e}") from None
+            intrin = torch.Tensor(cam_data["cam_intrinsic"])
+            sensor2lidar = torch.tensor(results["lidar2cam_dic"][cam_name]).inverse().float()
+            resize, resize_dims, crop = self.sample_augmentation(H, W)
+            post_rot, post_tran = self.post_homography(resize, crop)
+            files.append(data)
+            paths.append(path)
+            sizes.append((H, W))
+            intrins.append(intrin)
+            rots.append(sensor2lidar[:3, :3])
+            trans.append(sensor2lidar[:3, 3])
+            post_rots.append(post_rot)
+            post_trans.append(post_tran)
+            sensor2sensors.append(sensor2lidar)
+            dims.append(resize_dims)
+            crops.append(crop)
+        if len(set(sizes)) != 1:
+            raise ValueError("LoadMultiViewJpegBytes_OccFormer: the cameras of a sample need one frame size")
+        gt_depths = [torch.zeros(1) for _ in cam_names]
+        results["img_inputs"] = (torch.zeros((len(cam_names), 0), dtype=torch.uint8),) + tuple(
+            torch.stack(x) for x in (rots, trans, intrins, post_rots, post_trans, gt_depths, sensor2sensors))
+        results["img_aug"] = dict(self.img_aug(dims, crops), jpeg=files, jpeg_files=paths)
         return results
