@@ -488,6 +488,18 @@ int occ_lidarseg_occupancy(const float* pts, int ld, const long long* offsets /*
                            int panoptic, long long empty_id, long long ignore, int* invalid, void* ws, size_t ws_bytes,
                            long long* out, occ_stream_t stream);
 
+/* SemanticKITTI occupancy ground truth from the dataset's voxel files (csrc/semkitti_labels.cu), replacing the offline
+ *   semantic_kitti_preprocess.main _1_1 volume    P/tools/kitti_process/semantic_kitti_preprocess.py:117-142
+ * and LoadSemKittiAnnotation's torch.tensor(np.load(...)).long() (P/datasets/pipelines/loading_kitti_occ.py:34-53).
+ * label: B samples of nvox uint16 little-endian values (the .label files' bytes, sample b at b * 2 * nvox), 16-byte
+ * aligned; invalid: B samples of nvox / 8 bytes (the .invalid files, bit-packed, most significant bit first,
+ * io_data.unpack); nvox % 8 == 0, 1 <= B <= 65536.  lut: lut_size int32 values, the remap LUT as io_data.get_remap_lut
+ * builds it.  out (B, nvox) int64, 16-byte aligned, overwritten: lut[label], then 255 where the invalid bit is set.  A
+ * label >= lut_size (the reference's numpy IndexError) adds to bad[b] (B device ints, ACCUMULATED) and is written as
+ * 255; nothing is read or written out of bounds.  One launch per call, no host synchronisation. */
+int occ_semkitti_labels(const unsigned char* label, const unsigned char* invalid, int B, long long nvox,
+                        const int* lut, int lut_size, int* bad, long long* out, occ_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------------------
  * Camera images from the decoded frames (csrc/image_prep.cu): steps 2-4 of the test loaders' image side,
  *   LoadMultiViewImageFromFiles_OccFormer     P/datasets/pipelines/loading_nusc_imgs.py:34-62,181-195

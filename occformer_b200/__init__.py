@@ -14,6 +14,6 @@ from .head import (Mask2FormerNuscOccHead, Mask2FormerNuscPanopticOccHead, Mask2
 from .detector import OccupancyFormer  # noqa: F401
 from .pipelines import (LoadMultiViewImageFrames_OccFormer, LoadMultiViewImageFrames_SemanticKitti,  # noqa: F401
                         LoadMultiViewJpegBytes_OccFormer,
-                        LoadNuscOccupancyPoints, LoadNuscPanopticOccupancyPoints)
+                        LoadNuscOccupancyPoints, LoadNuscPanopticOccupancyPoints, LoadSemKittiVoxelFiles)
 
 __version__ = "0.1.0"

@@ -24,7 +24,7 @@ import torch
 import torch.nn as nn
 
 from . import dist_eval, image_prep, targets
-from .head import Mask2FormerNuscOccHead, Mask2FormerNuscPanopticOccHead
+from .head import Mask2FormerNuscOccHead, Mask2FormerNuscPanopticOccHead, Mask2FormerOccHead
 from .image_encoder import SECONDFPN, ResNet, ResNetDCN
 from .registry import BACKBONES, DETECTORS, HEADS, NECKS
 
@@ -39,6 +39,11 @@ def _build(registry, cfg, default_args=None):
     elif cfg.get("type") == "SECONDFPN":
         cfg["type"] = SECONDFPN
     return registry.build(cfg, default_args)
+
+
+def _voxel_files(img_metas):
+    """every sample's metas carry the SemanticKITTI voxel files of pipelines.LoadSemKittiVoxelFiles"""
+    return bool(img_metas) and all("semkitti_voxels" in m for m in img_metas)
 
 
 def _pts(cfg):
@@ -164,12 +169,16 @@ class OccupancyFormer(nn.Module):
     @torch.no_grad()
     def simple_test(self, img_metas, img=None, rescale=False, points_occ=None, gt_occ=None, points_uv=None):
         """occupancyformer.py:209-237 -> the head's dict with 'output_voxels' (B, K, *occ_size) and 'target_voxels' = gt_occ;
-        with LiDAR points also 'output_points' (int64 labels), 'target_points' and 'evaluation_semantic'.
+        with LiDAR points also 'output_points' (int64 labels), 'target_points' and 'evaluation_semantic'.  Without gt_occ,
+        the SemanticKITTI head builds 'target_voxels' from the voxel files of LoadSemKittiVoxelFiles when every sample's
+        metas carry 'semkitti_voxels' (occupancy_targets).
 
         The panoptic head's dict is returned as the head makes it, plus 'target_voxels' and 'target_points': its
         'output_voxels' is [(semantic, panoptic)] and its 'output_points' are labels already, which the reference detector
         cannot take (INTEGRATION.md)."""
         if gt_occ is None and points_occ is not None and self.occ_targets_from_points:
+            gt_occ = self.occupancy_targets(points_occ, img_metas)
+        elif gt_occ is None and _voxel_files(img_metas) and isinstance(self.pts_bbox_head, Mask2FormerOccHead):
             gt_occ = self.occupancy_targets(points_occ, img_metas)
         voxel_feats, img_feats, depth = self.extract_feat(points=None, img=img, img_metas=img_metas)
         output = self.pts_bbox_head.simple_test(voxel_feats=voxel_feats, points=points_occ, img_metas=img_metas,
@@ -194,15 +203,24 @@ class OccupancyFormer(nn.Module):
         """The gt_occ the reference's nuScenes loader builds for these points (occformer_b200.targets), on their device:
         points_occ = list of per-sample (n_i, 4) CUDA tensors [x, y, z, label | panoptic id], occ_size and pc_range from
         img_metas[0] -> int64 (B, X, Y, Z): semantic labels for Mask2FormerNuscOccHead, panoptic ids for
-        Mask2FormerNuscPanopticOccHead.  Reads one invalid-point count back to the host (ValueError if nonzero)."""
+        Mask2FormerNuscPanopticOccHead.  Reads one invalid-point count back to the host (ValueError if nonzero).
+        Mask2FormerOccHead (SemanticKITTI): points_occ is unused; every sample's img_metas carry the 'semkitti_voxels' of
+        LoadSemKittiVoxelFiles -> int64 (B, 256, 256, 32) from those files (targets.semantic_kitti_occupancy)."""
         head = self.pts_bbox_head
         if isinstance(head, Mask2FormerNuscPanopticOccHead):
             build = targets.panoptic_occupancy
         elif isinstance(head, Mask2FormerNuscOccHead):
             build = targets.lidarseg_occupancy
+        elif isinstance(head, Mask2FormerOccHead) and _voxel_files(img_metas):
+            vox = [m["semkitti_voxels"] for m in img_metas]
+            if any(v["learning_map"] != vox[0]["learning_map"] for v in vox[1:]):
+                raise ValueError("occupancy_targets: every sample of a batch needs the same learning map")
+            return targets.semantic_kitti_occupancy([v["label"] for v in vox], [v["invalid"] for v in vox],
+                                                    vox[0]["learning_map"], names=[v["files"] for v in vox])
         else:
             raise NotImplementedError(f"occupancy_targets: {type(head).__name__} scores against preprocessed voxel labels "
-                                      "(SemanticKITTI), not a LiDAR point scan; pass gt_occ")
+                                      "(SemanticKITTI), not a LiDAR point scan; pass gt_occ, or the voxel files of "
+                                      "LoadSemKittiVoxelFiles ('semkitti_voxels' in every sample's metas)")
         # the reference's datasets store both fields as numpy arrays (nuscenes_lss_dataset.py:86-87), configs as lists
         occ_size, pc_range = (np.asarray(img_metas[0][k]) for k in ("occ_size", "pc_range"))
         same = (np.array_equal(np.asarray(m["occ_size"]), occ_size) and np.array_equal(np.asarray(m["pc_range"]), pc_range)

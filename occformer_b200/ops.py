@@ -978,6 +978,16 @@ def lidarseg_occupancy(pts, counts, pc_range, grid, panoptic, empty_id, ignore):
     return out, invalid
 
 
+def semkitti_labels(label, invalid, B, nvox, lut):
+    """SemanticKITTI ground truth of B samples (occ_semkitti_labels): label uint8 CUDA (B * 2 * nvox,) bytes of the
+    .label files, invalid uint8 CUDA (B * nvox / 8,) bytes of the .invalid files, lut int32 CUDA remap table ->
+    (int64 (B, nvox) volume, int32 (B,) count of labels past the LUT per sample); no synchronisation."""
+    out = torch.empty((B, nvox), dtype=torch.int64, device=label.device)
+    bad = torch.zeros(B, dtype=torch.int32, device=label.device)
+    _call("occ_semkitti_labels", label, invalid, B, nvox, lut, lut.numel(), bad, out)
+    return out, bad
+
+
 # ----------------------------------------------------------------------------------------------- camera images
 _prep_tables = {}  # (device, source size, resized size) -> int32 resample table of one axis (image_prep.resample_table)
 _prep_norms = {}   # (device, mean, std, to_rgb) -> float32 (3, 256) normalisation table

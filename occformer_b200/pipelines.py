@@ -1,6 +1,7 @@
 """Loader transforms that leave the occupancy ground truth (occformer_b200.targets), the camera images' resize, crop and
 normalisation (occformer_b200.image_prep, the LoadMultiViewImageFrames_* transforms) or also the JPEG decoding
-(LoadMultiViewJpegBytes_OccFormer, at the end of this file) to the GPU.
+(LoadMultiViewJpegBytes_OccFormer) to the GPU.  LoadSemKittiVoxelFiles, at the end of this file, hands SemanticKITTI's
+voxel files to the GPU in place of the preprocessed labels.
 
     LoadNuscOccupancyPoints          = LoadNuscOccupancyAnnotations          P/datasets/pipelines/loading_nusc_occ.py:13-120
     LoadNuscPanopticOccupancyPoints  = LoadNuscPanopticOccupancyAnnotations  P/datasets/pipelines/loading_nusc_panoptic_occ.py:32-145
@@ -276,4 +277,43 @@ class LoadMultiViewJpegBytes_OccFormer(LoadMultiViewImageFrames_OccFormer):
         results["img_inputs"] = (torch.zeros((len(cam_names), 0), dtype=torch.uint8),) + tuple(
             torch.stack(x) for x in (rots, trans, intrins, post_rots, post_trans, gt_depths, sensor2sensors))
         results["img_aug"] = dict(self.img_aug(dims, crops), jpeg=files, jpeg_files=paths)
+        return results
+
+
+# ---------------------------------------------------------------------------------------------- SemanticKITTI labels
+@PIPELINES.register_module()
+class LoadSemKittiVoxelFiles:
+    """The SemanticKITTI ground truth from the dataset's own voxel files instead of the preprocessed '<frame>_1_1.npy'
+    (tools/kitti_process/semantic_kitti_preprocess.py): reads dataset/sequences/{sequence}/voxels/{frame_id}.label and
+    .invalid under data_root, and the learning map from the dataset yaml at data_info_path (the file the preprocessing
+    step takes).  results['semkitti_voxels'] = dict(label=, invalid= (the files' bytes), files= (their paths),
+    learning_map=); results['gt_occ'] = None, so a following LoadSemKittiAnnotation takes its test-mode path and the
+    npy the dataset may have loaded is dropped.  OccupancyFormer.simple_test then builds 'target_voxels' on the GPU
+    (targets.semantic_kitti_occupancy); 'semkitti_voxels' must be collected into the img_metas (Collect3D meta_keys).
+    Files of the wrong size raise ValueError here, in the loader.  Test pipelines only: before a training-mode
+    LoadSemKittiAnnotation the None would silently skip its augmentation and its gt_occ, so is_train=True (the
+    annotation transform's flag, repeated here) is refused."""
+
+    def __init__(self, data_root="data/SemanticKITTI", data_info_path="projects/configs/_base_/semantickitti.yaml",
+                 is_train=False):
+        if is_train:
+            raise ValueError("LoadSemKittiVoxelFiles: is_train=True is not supported: the transform hands no gt_occ to "
+                             "LoadSemKittiAnnotation, whose training path needs it for the augmentation; keep the "
+                             "preprocessed labels for training pipelines")
+        import yaml
+        with open(data_info_path, "r") as f:
+            self.learning_map = yaml.safe_load(f)["learning_map"]
+        self.data_root, self.data_info_path = data_root, data_info_path
+
+    def __call__(self, results):
+        from .targets import SEMKITTI_INVALID_BYTES, SEMKITTI_LABEL_BYTES
+        base = os.path.join(self.data_root, "dataset", "sequences", results["sequence"], "voxels", results["frame_id"])
+        files, data = [base + ".label", base + ".invalid"], []
+        for path, size in zip(files, (SEMKITTI_LABEL_BYTES, SEMKITTI_INVALID_BYTES)):
+            with open(path, "rb") as f:
+                data.append(f.read())
+            if len(data[-1]) != size:
+                raise ValueError(f"{path}: a SemanticKITTI voxel file of {size} bytes is needed, got {len(data[-1])}")
+        results["semkitti_voxels"] = dict(label=data[0], invalid=data[1], files=files, learning_map=self.learning_map)
+        results["gt_occ"] = None
         return results

@@ -9,7 +9,16 @@ the mapped label (semantic) or id (panoptic) in column 3, an integer below 2^24 
 (occ_lidarseg_occupancy, csrc/occ_targets.cu) voxelises in float64 as numpy does and takes each voxel's majority id with
 no sort.  Out-of-contract points (a label that is negative, not an integer or at or above 256 / 65536, a non-finite
 coordinate, more than 65535 points of one id in one voxel) raise ValueError; there is no CPU fallback.
+
+SemanticKITTI's ground truth comes from the dataset's own voxel files instead of the offline preprocessing step:
+
+    semantic_kitti_occupancy   semantic_kitti_preprocess.main (_1_1)  P/tools/kitti_process/semantic_kitti_preprocess.py:117-142
+                               + LoadSemKittiAnnotation's .long()     P/datasets/pipelines/loading_kitti_occ.py:34-53
+
+The 4 MB .label and 256 KB .invalid files of a frame cross PCIe instead of the 16 MB int64 volume, and the kernel
+(occ_semkitti_labels, csrc/semkitti_labels.cu) remaps and masks them in one pass.
 """
+import numpy as np
 import torch
 
 from . import ops
@@ -55,3 +64,85 @@ def panoptic_occupancy(points, occ_size, point_cloud_range, unoccupied_id=17):
     int64 (B, X, Y, Z) (or (X, Y, Z)): each occupied voxel's majority id without id 0 (which still decides the voxel the
     reference writes last, as its loader does), 0 -> 65535, unoccupied_id * 1000 -> 0, empty voxels 0."""
     return _occupancy(points, occ_size, point_cloud_range, 1, int(unoccupied_id * 1e3), PANOPTIC_IGNORE)
+
+
+# ---------------------------------------------------------------------------------------------- SemanticKITTI
+SEMKITTI_SHAPE = (256, 256, 32)
+SEMKITTI_LABEL_BYTES = 2 * 256 * 256 * 32   # .label: one uint16 per voxel
+SEMKITTI_INVALID_BYTES = 256 * 256 * 32 // 8  # .invalid: one bit per voxel
+_semkitti_luts = {}  # (device, LUT bytes) -> int32 CUDA remap table
+_semkitti_staging = {}  # device -> (grow-only pinned uint8 buffer, CUDA event after its last host-to-device copy)
+
+
+def semkitti_remap_lut(learning_map):
+    """io_data.get_remap_lut (P/tools/kitti_process/io_data.py:173-193) from the dataset yaml's learning_map -> int32
+    numpy table of max key + 100 entries: learning_map[k], 255 for keys the map lacks or maps to 0, 0 for key 0."""
+    keys = [int(k) for k in learning_map]
+    if not keys or min(keys) < 0 or max(keys) + 100 > 65536:
+        raise ValueError("semkitti_remap_lut: learning_map keys must be labels in [0, 65436)")
+    lut = np.zeros(max(keys) + 100, dtype=np.int32)
+    lut[keys] = [int(v) for v in learning_map.values()]
+    lut[lut == 0] = 255
+    lut[0] = 0
+    return lut
+
+
+def _bytes(x, size, what, name):
+    m = memoryview(x).cast("B")
+    if m.nbytes != size:
+        raise ValueError(f"semantic_kitti_occupancy: {name}: a {what} file holds {size} bytes, got {m.nbytes}")
+    return m
+
+
+def semantic_kitti_occupancy(labels, invalids, learning_map, names=None):
+    """SemanticKITTI occupancy ground truth from the voxel files: labels / invalids = the bytes (bytes-like) of one
+    sample's voxels/*.label and voxels/*.invalid, or lists of B of each; learning_map = the dataset yaml's -> int64 CUDA
+    (256, 256, 32) (or (B, 256, 256, 32)) on the current device, equal to the reference's
+    torch.tensor(np.load('<frame>_1_1.npy')).long(): remap_lut[label], then 255 where the invalid bit is set.  The files
+    travel in one host-to-device copy from a pinned staging buffer kept per device.  A file of the wrong size, or a label
+    at or past the LUT (the reference's IndexError; one count read back), raises ValueError naming the file (names: B
+    (.label name, .invalid name) pairs for the messages; default: the sample index)."""
+    single = not isinstance(labels, (list, tuple))
+    labels = [labels] if single else list(labels)
+    invalids = [invalids] if single else list(invalids)
+    B = len(labels)
+    if B == 0 or len(invalids) != B:
+        raise ValueError("semantic_kitti_occupancy: needs one .label and one .invalid file per sample")
+    names = [tuple(n) for n in names] if names is not None else [(f"sample {b}",) * 2 for b in range(B)]
+    if len(names) != B or any(len(n) != 2 for n in names):
+        raise ValueError("semantic_kitti_occupancy: names are B (.label name, .invalid name) pairs")
+    lab = [_bytes(x, SEMKITTI_LABEL_BYTES, ".label", n[0]) for x, n in zip(labels, names)]
+    inv = [_bytes(x, SEMKITTI_INVALID_BYTES, ".invalid", n[1]) for x, n in zip(invalids, names)]
+    lut = semkitti_remap_lut(learning_map)
+    if not torch.cuda.is_available():
+        raise RuntimeError("occformer_b200.targets: semantic_kitti_occupancy needs a CUDA device (no CPU fallback exists)")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    key = (str(dev), lut.tobytes())
+    lut_d = _semkitti_luts.get(key)
+    if lut_d is None:
+        lut_d = torch.from_numpy(lut).to(dev)
+        _semkitti_luts[key] = lut_d
+    split = B * SEMKITTI_LABEL_BYTES
+    total = split + B * SEMKITTI_INVALID_BYTES
+    staging, copied = _semkitti_staging.get(str(dev), (None, None))
+    if staging is None or staging.numel() < total:
+        staging, copied = torch.empty(total, dtype=torch.uint8, pin_memory=True), torch.cuda.Event()
+    copied.synchronize()  # the buffer's previous copy has left it (a no-op after the read-back of a finished call)
+    host = staging[:total]
+    hv = host.numpy()
+    for b in range(B):
+        hv[b * SEMKITTI_LABEL_BYTES:(b + 1) * SEMKITTI_LABEL_BYTES] = np.frombuffer(lab[b], np.uint8)
+        o = split + b * SEMKITTI_INVALID_BYTES
+        hv[o:o + SEMKITTI_INVALID_BYTES] = np.frombuffer(inv[b], np.uint8)
+    data = host.to(dev, non_blocking=True)
+    copied.record()
+    _semkitti_staging[str(dev)] = (staging, copied)
+    nvox = SEMKITTI_LABEL_BYTES // 2
+    vol, bad = ops.semkitti_labels(data[:split], data[split:], B, nvox, lut_d)
+    bad = bad.cpu()  # the one host synchronisation
+    if bool(bad.any()):
+        b = int(bad.nonzero()[0, 0])
+        raise ValueError(f"semantic_kitti_occupancy: {names[b][0]}: {int(bad[b])} voxel labels are at or past the remap "
+                         f"table's {lut.size} entries (the learning map's largest key + 100)")
+    vol = vol.view(B, *SEMKITTI_SHAPE)
+    return vol[0] if single else vol
