@@ -70,7 +70,8 @@ CONV_CASES = [
     # few output tiles, long K: split-K (partial sums meet through TMA reduce-add, GroupNorm statistics from the result)
     (1, 25, 25, 4, 256, 512, (3, 3, 3), 1, 1),
     (2, 50, 50, 8, 128, 256, (3, 3, 3), 2, 1),
-    # many M-tiles, N <= 128: paired M-tiles share the weight k-blocks (MT = 2); 611 tiles = odd tail pair
+    # many M-tiles, short K: 611 128-row tiles (1 x 4 x 32 voxel boxes) at BN 64, more than four per SM (27 k-blocks
+    # and BN 64 keep it off the 256-row tiles, which need BN 96 / 128 and at least 64 k-blocks)
     (1, 47, 51, 32, 32, 64, (3, 3, 3), 1, 1),
     # group sizes that are not powers of two: 192 channels / 32 groups (cpg 6) in the epilogue, 96 / 32 (cpg 3) split-K
     (1, 20, 20, 4, 64, 192, (3, 3, 3), 1, 1),
