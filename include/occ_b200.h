@@ -565,6 +565,41 @@ int occ_decode_jpeg(const unsigned char* data, long long data_bytes, const long 
                     int M, int seq_bits, int sync_rounds, void* ws, size_t ws_bytes, unsigned char* out,
                     long long out_bytes, int* status, occ_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * Camera frames from their PNG files (csrc/png_decode.cu): step 1 of the SemanticKITTI test loader's image side,
+ *   LoadMultiViewImageFromFiles_SemanticKitti  P/datasets/pipelines/loading_kitti_imgs.py:103 (mmcv.imread, cv2)
+ * bit for bit as cv2.imdecode(buf, IMREAD_UNCHANGED) with libpng and zlib: 8-bit RGB, non-interlaced, DEFLATE with
+ * stored, fixed and dynamic Huffman blocks, the five PNG filter types.  occformer_b200/png.py walks the chunks and
+ * refuses everything else on the host.
+ *   data         uint8, data_bytes bytes, holding the zlib streams (each image's IDAT payloads back to back)
+ *   streams      HOST int64 (M): byte offset in data of image m's zlib stream (from its 2-byte header)
+ *   geom         HOST int32 (M, 4): H, W (1..16384), stream bytes (7 .. 2^27 - 1; offset + bytes <= data_bytes),
+ *                CINFO of the zlib header (0..7)
+ *   idat_counts  HOST int32 (M): IDAT chunks of image m (1 .. stream bytes)
+ *   idat         int32, idat_len entries: per image in order, the stream offset at which each IDAT chunk's payload
+ *                starts (the first is 0).  libpng hands zlib each chunk in reads of 8192 bytes, which decides whether a
+ *                wrong Adler-32 fails the image (status 4)
+ *   out_offsets  HOST int64 (M): byte offset of image m's (H, W, 3) uint8 B, G, R frame in out (out_bytes bytes); only
+ *                those bytes of out are written
+ *   status       (M, 2) int32, overwritten: status[m, 0] = 0 where cv2 decodes the image, else the OR of 1 (invalid
+ *                DEFLATE data that zlib meets while libpng reads the rows: before the rows are complete, or an
+ *                invalid code or block header right after the last row's byte in the same read), 2 (the stream ends
+ *                early, or inflates to fewer than H (1 + 3W) bytes), 4 (an Adler-32 mismatch libpng meets while
+ *                reading the rows), 8 (a filter type above 4); status[m, 1] = blocks decoded serially while linking.
+ *                Errors zlib meets only after the rows (libpng's benign "too much image data" and later checks) and
+ *                bytes after the end of the stream are ignored, as libpng ignores them.  The frame of a failed image
+ *                is undefined, but nothing is written outside it.
+ *   ws           occ_decode_png_workspace_bytes(streams, geom, idat_counts, M) bytes, 16-byte aligned
+ * 1 <= M <= 96.  37 enqueued launches and memsets per call (7 + 30 pointer-jumping rounds) whatever M and the data, no
+ * host synchronisation (capturable in a CUDA graph).  Returns -1 for a bad M, geometry, stream, IDAT count, output
+ * range, a short idat array or a short or misaligned workspace, with nothing enqueued. */
+size_t occ_decode_png_workspace_bytes(const long long* streams /*HOST*/, const int* geom /*HOST*/,
+                                      const int* idat_counts /*HOST*/, int M);
+int occ_decode_png(const unsigned char* data, long long data_bytes, const long long* streams /*HOST*/,
+                   const int* geom /*HOST*/, const int* idat_counts /*HOST*/, const int* idat, long long idat_len,
+                   const long long* out_offsets /*HOST*/, int M, void* ws, size_t ws_bytes, unsigned char* out,
+                   long long out_bytes, int* status, occ_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

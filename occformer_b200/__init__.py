@@ -13,7 +13,7 @@ from .head import (Mask2FormerNuscOccHead, Mask2FormerNuscPanopticOccHead, Mask2
                    SinePositionalEncoding3D)
 from .detector import OccupancyFormer  # noqa: F401
 from .pipelines import (LoadMultiViewImageFrames_OccFormer, LoadMultiViewImageFrames_SemanticKitti,  # noqa: F401
-                        LoadMultiViewJpegBytes_OccFormer,
+                        LoadMultiViewJpegBytes_OccFormer, LoadMultiViewPngBytes_SemanticKitti,
                         LoadNuscOccupancyPoints, LoadNuscPanopticOccupancyPoints, LoadSemKittiVoxelFiles)
 
 __version__ = "0.1.0"

@@ -122,16 +122,20 @@ class OccupancyFormer(nn.Module):
         imgs may also be the uint8 (B, N, H, W, 3) BGR frames of occformer_b200.pipelines' LoadMultiViewImageFrames_*
         transforms: they are resized, cropped and normalised on the GPU first (image_prep.prepare_images), from the
         'img_aug' of each sample's metas.  An empty uint8 (B, N, 0) imgs is LoadMultiViewJpegBytes_OccFormer's
-        placeholder: the JPEG files in each 'img_aug' are decoded on the GPU first (image_prep.decode_jpeg)."""
+        placeholder: the JPEG files in each 'img_aug' are decoded on the GPU first (image_prep.decode_jpeg); so is
+        LoadMultiViewPngBytes_SemanticKitti's (B, 1, 0) one, whose 'img_aug' carries PNG files (image_prep.decode_png)."""
         imgs = img[0]
         if torch.is_tensor(imgs) and imgs.dtype == torch.uint8 and imgs.dim() == 3 and imgs.shape[-1] == 0:
-            if img_metas is None or any("jpeg" not in m.get("img_aug", {}) for m in img_metas):
+            augs = [m.get("img_aug", {}) for m in img_metas] if img_metas is not None else []
+            kind = next((k for k in ("png", "jpeg") if augs and all(k in a for a in augs)), None)
+            if kind is None:
                 raise ValueError("OccupancyFormer: the empty image placeholder needs each sample's 'img_aug' meta with "
-                                 "its 'jpeg' files, which LoadMultiViewJpegBytes_OccFormer produces; add 'img_aug' to "
-                                 "Collect3D's meta_keys")
-            augs = [m["img_aug"] for m in img_metas]
-            names = [a.get("jpeg_files") for a in augs]
-            imgs = image_prep.decode_jpeg([a["jpeg"] for a in augs], None if None in names else names)
+                                 "its 'jpeg' files, which LoadMultiViewJpegBytes_OccFormer produces, or its 'png' files, "
+                                 "which LoadMultiViewPngBytes_SemanticKitti produces; add 'img_aug' to Collect3D's "
+                                 "meta_keys")
+            names = [a.get(kind + "_files") for a in augs]
+            decode = image_prep.decode_png if kind == "png" else image_prep.decode_jpeg
+            imgs = decode([a[kind] for a in augs], None if None in names else names)
         if (imgs.dtype if torch.is_tensor(imgs) else imgs[0].dtype) == torch.uint8:
             if img_metas is None or any("img_aug" not in m for m in img_metas):
                 raise ValueError("OccupancyFormer: uint8 camera frames need each sample's 'img_aug' meta, which the "

@@ -9,7 +9,8 @@ The loader transforms of occformer_b200.pipelines hand the model uint8 BGR frame
 
 decode_jpeg decodes the camera files themselves on the device (csrc/jpeg_decode.cu), bit for bit as cv2.imdecode,
 into the frames prepare_images takes; the loader then ships the JPEG bytes instead of the decoded frames
-(pipelines.LoadMultiViewJpegBytes_OccFormer).
+(pipelines.LoadMultiViewJpegBytes_OccFormer).  decode_png does the same for SemanticKITTI's PNG frames
+(csrc/png_decode.cu, pipelines.LoadMultiViewPngBytes_SemanticKitti).
 
 The host part here is table building: Pillow's bicubic coefficients per (source size, resized size) of an axis and the
 normalisation as a 3 x 256 table, both in float64 numpy, one operation at a time as x86-64 builds of Pillow and OpenCV
@@ -20,7 +21,7 @@ import math
 import numpy as np
 import torch
 
-from . import jpeg, ops
+from . import jpeg, ops, png
 
 PRECISION_BITS = 22  # Pillow's resample.c: 32 - 8 - 2
 DEFAULT_NORM = dict(mean=[123.675, 116.28, 103.53], std=[58.395, 57.12, 57.375], to_rgb=True)  # mmlabNormalize's
@@ -147,13 +148,8 @@ def decode_jpeg(files, names=None, seq_bits=ops.JPEG_SEQ_BITS, sync_rounds=ops.J
         sizes = {(h.height, h.width) for h in headers[b0:b0 + len(s)]}
         if len(sizes) != 1:
             raise ValueError(f"decode_jpeg: the cameras of a sample need one frame size, got {sorted(sizes)}")
-    offsets = np.cumsum([0] + [len(f) for f in flat]).tolist()
-    host = torch.empty(offsets[-1], dtype=torch.uint8, pin_memory=True)
-    hv = host.numpy()
-    for f, o in zip(flat, offsets):
-        hv[o:o + len(f)] = np.frombuffer(f, np.uint8)
-    data = host.to(torch.cuda.current_device(), non_blocking=True)
-    out, status = ops.decode_jpeg(data, offsets[:-1], headers, seq_bits, sync_rounds)
+    data, offsets = _stage(flat)
+    out, status = ops.decode_jpeg(data, offsets, headers, seq_bits, sync_rounds)
     bad = status[:, 0].cpu()
     if bool(bad.any()):
         m = int(bad.nonzero()[0, 0])
@@ -163,6 +159,23 @@ def decode_jpeg(files, names=None, seq_bits=ops.JPEG_SEQ_BITS, sync_rounds=ops.J
                          + ", ".join(w for bit, w in ((1, "unexpected marker"), (2, "bad restart markers"),
                                                       (4, "invalid Huffman code or run"), (8, "data ends early"))
                                      if int(bad[m]) & bit) + ")")
+    return _frames(out, samples, headers)
+
+
+def _stage(pieces):
+    """bytes-like pieces -> (uint8 CUDA buffer holding them back to back, each piece's byte offset): one pinned host
+    buffer and one host-to-device copy"""
+    offsets = np.cumsum([0] + [len(f) for f in pieces]).tolist()
+    host = torch.empty(offsets[-1], dtype=torch.uint8, pin_memory=True)
+    hv = host.numpy()
+    for f, o in zip(pieces, offsets):
+        hv[o:o + len(f)] = np.frombuffer(f, np.uint8)
+    return host.to(torch.cuda.current_device(), non_blocking=True), offsets[:-1]
+
+
+def _frames(out, samples, headers):
+    """the decoders' flat frames -> (B, N, H, W, 3) when every sample shares N and the frame size, else the list of B
+    per-sample (N, H_i, W_i, 3) views"""
     shapes = [(len(s), headers[b0].height, headers[b0].width)
               for s, b0 in zip(samples, np.cumsum([0] + [len(s) for s in samples])[:-1])]
     if len(set(shapes)) == 1 and len({len(s) for s in samples}) == 1:
@@ -172,3 +185,52 @@ def decode_jpeg(files, names=None, seq_bits=ops.JPEG_SEQ_BITS, sync_rounds=ops.J
         res.append(out[o:o + N * H * W * 3].view(N, H, W, 3))
         o += N * H * W * 3
     return res
+
+
+PNG_STATUS = ((1, "invalid deflate data"), (2, "data ends early or too little image data"),
+              (4, "incorrect Adler-32 check"), (8, "bad filter type"))
+
+
+def decode_png(files, names=None):
+    """files: B samples, each a list of N 8-bit RGB PNG files (bytes-like) -> uint8 CUDA (B, N, H, W, 3) B, G, R frames
+    when all share one size, else a list of B per-sample (N, H_i, W_i, 3) tensors: the two forms prepare_images takes,
+    equal to cv2.imdecode(buf, IMREAD_UNCHANGED) of each file.  png.parse walks the chunks on the host (refused kinds
+    raise ValueError naming the file); the zlib streams and the IDAT chunk starts travel in one pinned host buffer and
+    one host-to-device copy, and decode in one occ_decode_png call; one status read-back then raises ValueError naming
+    a file cv2 would not decode.  names: the same nesting of file names for the messages (default: sample and camera
+    indices)."""
+    samples = [list(s) for s in files]
+    if not samples or any(not s for s in samples):
+        raise ValueError("decode_png: needs at least one sample of at least one file")
+    label = [[names[b][n] if names is not None else f"sample {b} camera {n}" for n in range(len(s))]
+             for b, s in enumerate(samples)]
+    headers, pieces, starts = [], [], []
+    for s, lab in zip(samples, label):
+        for f, name in zip(s, lab):
+            try:
+                h = png.parse(f)
+            except png.PngError as e:
+                raise ValueError(f"decode_png: {name}: {e}") from None
+            headers.append(h)
+            v = memoryview(f).cast("B")
+            pieces += [v[o:o + n] for o, n in h.idat]
+            starts += np.cumsum([0] + [n for _, n in h.idat])[:-1].tolist()
+    for s, lab, b0 in zip(samples, label, np.cumsum([0] + [len(s) for s in samples])[:-1]):
+        sizes = {(h.height, h.width) for h in headers[b0:b0 + len(s)]}
+        if len(sizes) != 1:
+            raise ValueError(f"decode_png: the cameras of a sample need one frame size, got {sorted(sizes)}")
+    streams = sum((h.stream_len for h in headers), 0)
+    pad = -streams % 4
+    pieces += [bytes(pad), np.asarray(starts, np.int32).tobytes()]
+    data, offsets = _stage(pieces)
+    stream_off = np.cumsum([0] + [h.stream_len for h in headers])[:-1].tolist()
+    idat = data[streams + pad:].view(torch.int32)
+    out, status = ops.decode_png(data[:max(streams, 1)], stream_off, headers, idat)
+    bad = status[:, 0].cpu()
+    if bool(bad.any()):
+        m = int(bad.nonzero()[0, 0])
+        b = int(np.searchsorted(np.cumsum([len(s) for s in samples]), m, side="right"))
+        n = m - sum(len(s) for s in samples[:b])
+        raise ValueError(f"decode_png: {label[b][n]}: cv2 would not decode it (status {int(bad[m])}: "
+                         + ", ".join(w for bit, w in PNG_STATUS if int(bad[m]) & bit) + ")")
+    return _frames(out, samples, headers)

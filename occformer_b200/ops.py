@@ -1050,6 +1050,18 @@ def _jpeg_table(dev, key, table):
     return t
 
 
+def _stream_workspace(cache, dev, nbytes):
+    """the grow-only uint8 workspace of cache for the current stream of dev, at least nbytes long"""
+    key = (str(dev), torch.cuda.current_stream(dev).cuda_stream)
+    ent = cache.get(key)
+    if ent is None or ent[0].numel() < nbytes:
+        # a graph captured before the workspace grew still points at the old one: keep it referenced
+        old = [] if ent is None else ent[1] + [ent[0]]
+        ent = (torch.empty(nbytes, dtype=torch.uint8, device=dev), old)
+        cache[key] = ent
+    return ent[0]
+
+
 def decode_jpeg(data, offsets, headers, seq_bits=JPEG_SEQ_BITS, sync_rounds=JPEG_SYNC_ROUNDS):
     """M baseline JPEG files -> uint8 B, G, R frames (occ_decode_jpeg): data a flat uint8 CUDA buffer, file m at byte
     offsets[m], headers[m] = occformer_b200.jpeg.parse of it -> (out: flat uint8 CUDA buffer of the M (H, W, 3) frames
@@ -1073,17 +1085,44 @@ def decode_jpeg(data, offsets, headers, seq_bits=JPEG_SEQ_BITS, sync_rounds=JPEG
     nbytes = lib().occ_decode_jpeg_workspace_bytes(scan, geom, M, int(seq_bits))
     if nbytes == 0:
         raise RuntimeError(f"occformer_b200: occ_decode_jpeg takes 32 <= seq_bits <= 2^20, got {seq_bits}")
-    key = (str(dev), torch.cuda.current_stream(dev).cuda_stream)
-    ent = _jpeg_ws.get(key)
-    if ent is None or ent[0].numel() < nbytes:
-        # a graph captured before the workspace grew still points at the old one: keep it referenced
-        old = [] if ent is None else ent[1] + [ent[0]]
-        ent = (torch.empty(nbytes, dtype=torch.uint8, device=dev), old)
-        _jpeg_ws[key] = ent
-    ws = ent[0]
+    ws = _stream_workspace(_jpeg_ws, dev, nbytes)
     out = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)
     status = torch.empty((M, 2), dtype=torch.int32, device=dev)
     _call("occ_decode_jpeg", data, data.numel(), scan, geom, (ctypes.c_longlong * (9 * M))(*tables),
           (ctypes.c_longlong * M)(*out_off), M, int(seq_bits), int(sync_rounds), ws, ws.numel(), out, out.numel(),
           status)
+    return out[:total], status
+
+
+# ----------------------------------------------------------------------------------------------- PNG decoding
+PNG_MAX_IMAGES = 96     # images per occ_decode_png call
+PNG_LAUNCHES = 37       # enqueued launches and memsets per call (include/occ_b200.h)
+_png_ws = {}            # (device, stream) -> (grow-only uint8 workspace of occ_decode_png, superseded workspaces)
+
+
+def decode_png(data, offsets, headers, idat):
+    """M 8-bit RGB PNG files -> uint8 B, G, R frames (occ_decode_png): data a flat uint8 CUDA buffer holding image m's
+    zlib stream at byte offsets[m], headers[m] = occformer_b200.png.parse of the file, idat an int32 CUDA tensor of
+    every image's IDAT chunk starts in its stream (in image order) -> (out: flat uint8 CUDA buffer of the M (H, W, 3)
+    frames back to back, status: int32 CUDA (M, 2), see include/occ_b200.h).  No synchronisation."""
+    M = len(headers)
+    if not 1 <= M <= PNG_MAX_IMAGES:
+        raise ValueError(f"decode_png: 1 to {PNG_MAX_IMAGES} images per call, got {M}")
+    dev = data.device
+    geom, out_off, total = [], [], 0
+    for h in headers:
+        geom += [h.height, h.width, h.stream_len, h.cinfo]
+        out_off.append(total)
+        total += h.height * h.width * 3
+    streams = (ctypes.c_longlong * M)(*[int(o) for o in offsets])
+    geom = (ctypes.c_int * (4 * M))(*geom)
+    counts = (ctypes.c_int * M)(*[len(h.idat) for h in headers])
+    nbytes = lib().occ_decode_png_workspace_bytes(streams, geom, counts, M)
+    if nbytes == 0:
+        raise RuntimeError("occformer_b200: occ_decode_png refused the geometry or the streams")
+    ws = _stream_workspace(_png_ws, dev, nbytes)
+    out = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)
+    status = torch.empty((M, 2), dtype=torch.int32, device=dev)
+    _call("occ_decode_png", data, data.numel(), streams, geom, counts, idat, idat.numel(),
+          (ctypes.c_longlong * M)(*out_off), M, ws, ws.numel(), out, out.numel(), status)
     return out[:total], status

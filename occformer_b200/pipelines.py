@@ -280,6 +280,40 @@ class LoadMultiViewJpegBytes_OccFormer(LoadMultiViewImageFrames_OccFormer):
         return results
 
 
+@PIPELINES.register_module()
+class LoadMultiViewPngBytes_SemanticKitti(LoadMultiViewImageFrames_SemanticKitti):
+    """LoadMultiViewImageFrames_SemanticKitti without the decode: the frame file's bytes are read and the frame size
+    comes from its IHDR chunk (png.frame_size), so img_aug and img_inputs[1:] are the frame transform's.
+    results['img_aug'] also carries 'png' (the file's bytes, in a list of one) and 'png_files' (its path); img_inputs[0]
+    is an empty uint8 (1, 0) placeholder, which collates to (B, 1, 0).  OccupancyFormer then decodes the file on the GPU
+    (image_prep.decode_png) and prepares the image from the frame.  Files the device decoder does not take (16-bit,
+    grayscale, alpha, palette, tRNS, interlaced, animated, ...) raise ValueError here, in the loader.
+    results['raw_img'] needs the decoded frame on the host and is not produced: only the visualisation dump of the
+    test loop (pred_save) reads it, and that keeps the frame transform.  Test pipelines only: is_train=True is refused,
+    as the frame transform refuses it."""
+
+    def __call__(self, results):
+        from .png import PngError, frame_size
+        img_filenames = results["img_filename"]
+        assert len(img_filenames) == 1
+        path = img_filenames[0]
+        with open(path, "rb") as f:
+            data = f.read()
+        try:
+            H, W = frame_size(data)
+        except PngError as e:
+            raise ValueError(f"{path}: {e}") from None
+        resize, resize_dims, crop = self.sample_augmentation(H, W)
+        post_rot, post_tran = self.post_homography(resize, crop)
+        intrin = torch.Tensor(results["cam_intrinsic"][0])
+        lidar2cam = torch.Tensor(results["lidar2cam"][0])
+        cam2lidar = lidar2cam.inverse()
+        res = [cam2lidar[:3, :3], cam2lidar[:3, 3], intrin, post_rot, post_tran, torch.zeros(1), cam2lidar]
+        results["img_inputs"] = (torch.zeros((1, 0), dtype=torch.uint8),) + tuple(x[None] for x in res)
+        results["img_aug"] = dict(self.img_aug([resize_dims], [crop]), png=[data], png_files=[path])
+        return results
+
+
 # ---------------------------------------------------------------------------------------------- SemanticKITTI labels
 @PIPELINES.register_module()
 class LoadSemKittiVoxelFiles:
