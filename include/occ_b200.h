@@ -529,6 +529,46 @@ int occ_prepare_images(const unsigned char* frames, long long frame_bytes, const
                        const int* geom /*HOST*/, int M, int fH, int fW, const long long* tables /*HOST*/,
                        const float* norm, int swap_rb, void* ws, size_t ws_bytes, float* out, occ_stream_t stream);
 
+/* The training loaders' camera images (csrc/image_prep.cu): occ_prepare_images with the flip and rotation of
+ *   LoadMultiViewImageFromFiles_OccFormer(is_train=True).img_transform_core      P/datasets/pipelines/loading_nusc_imgs.py:55-62
+ *   LoadMultiViewImageFromFiles_SemanticKitti(is_train=True).img_transform_core  P/datasets/pipelines/loading_kitti_imgs.py:57-65
+ * bit for bit: resize and crop as above, then Image.transpose(FLIP_LEFT_RIGHT) when flipped, then Pillow's
+ * Image.rotate(angle) (NEAREST, no expand, black fill) of the fW x fH crop, then the normalisation table.
+ *   aug        HOST int32 (M, 7): flip (0 / 1), then a0..a5, the 16.16 fixed-point coefficients of Pillow's affine_fixed:
+ *              output pixel (x, y) reads crop pixel ((a2 + y a1 + x a0) >> 16, (a5 + y a4 + x a3) >> 16) of the
+ *              (mirrored) crop and takes 0 outside it.  occformer_b200.image_prep.rotate_coeffs computes them, also for
+ *              the angles where Pillow copies or transposes instead (0, 180, and 90 / 270 of a square crop).  At the
+ *              crop's corners a2 + y a1 + x a0 and a5 + y a4 + x a3 must fit in int32.
+ * Every other argument, the workspace (occ_prepare_images_workspace_bytes) and the errors are occ_prepare_images';
+ * a flip other than 0 / 1 or coefficients past int32 also return -1.  Two kernel launches per call whatever M, no
+ * memset, no host synchronisation; nothing is enqueued on an error. */
+int occ_prepare_images_aug(const unsigned char* frames, long long frame_bytes, const long long* offsets /*HOST*/,
+                           const int* geom /*HOST*/, const int* aug /*HOST*/, int M, int fH, int fW,
+                           const long long* tables /*HOST*/, const float* norm, int swap_rb, void* ws, size_t ws_bytes,
+                           float* out, occ_stream_t stream);
+
+/* Depth maps from the LiDAR scan (csrc/lidar_depth.cu): the gt_depths of
+ *   CreateDepthFromLiDAR   P/datasets/pipelines/lidar2depth.py:15-82
+ * bit for bit as the reference computes them with one torch thread (a DataLoader worker).  For each point p of sample
+ * b and camera n, in fp32, each dot product summed left to right without fused multiply-adds:
+ *   c = inv_rot (p - trans);  (x, y, d) = rows 0..2 of K c (K 4 x 4: of K (c, 1));  u = x / d, v = y / d;
+ *   (u', v') = post_rot[:2, :2] (u, v) + post_tran[:2];
+ * a point with u' >= 0, v' >= 0, u' <= fW - 1, v' <= fH - 1 and d > 0 (false for NaN) lands on pixel
+ * (rint(v'), rint(u')), round half to even.  Each pixel holds the smallest d that lands on it, else 0 (the reference's
+ * descending sort and last write win with one thread; with several its index_put_ picks any).
+ *   pts         float (n, 3), sample b's points at rows [offsets[b], offsets[b + 1]); NULL allowed when n = 0
+ *   offsets     HOST int64 (B + 1): offsets[0] = 0, non-decreasing, 1 <= B <= 256
+ *   inv_rots    float (B, N, 3, 3): rots.inverse() computed on the host in CPU fp32, as the reference does
+ *   trans       float (B, N, 3);  intrins float (B, N, k, k), k = intrin_dim = 3 or 4
+ *   post_rots   float (B, N, 3, 3);  post_trans float (B, N, 3)
+ *   out         float (B, N, fH, fW), overwritten
+ * 1 <= N <= 65535, fH, fW >= 1, fH * fW <= 2^31.  Three enqueued launches and memsets per call whatever the scans,
+ * deterministic, no host synchronisation (capturable in a CUDA graph).  Returns -1 for a bad count, size or offset,
+ * with nothing enqueued. */
+int occ_lidar_depth(const float* pts, const long long* offsets /*HOST*/, int B, int N, const float* inv_rots,
+                    const float* trans, const float* intrins, int intrin_dim, const float* post_rots,
+                    const float* post_trans, int fH, int fW, float* out, occ_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------------------
  * Camera frames from their JPEG files (csrc/jpeg_decode.cu): step 1 of the test loaders' image side,
  *   LoadMultiViewImageFromFiles_OccFormer     P/datasets/pipelines/loading_nusc_imgs.py:181-195 (mmcv.imread, cv2)

@@ -12,6 +12,11 @@
 //   vpass  per output pixel of the crop: (1 << 21) + sum w * p down the planes (0 outside the resized image), clipped
 //          >> 22, then norm[c][v] -> float NCHW
 // Two launches per call whatever M; the per-image descriptors travel in the kernel parameters (up to 256 images).
+//
+// occ_prepare_images_aug adds the training loaders' flip and rotation (img_transform_core: resize, crop, FLIP_LEFT_RIGHT,
+// Image.rotate).  Both only move pixels inside the crop window, so hpass is unchanged; vpass_aug maps each output pixel
+// through Pillow's 16.16 fixed-point nearest gather, the mirror and the crop offset to a resized (row, column), and
+// reads that row's vertical taps per thread.
 #include "occ_common.cuh"
 
 namespace occ {
@@ -116,6 +121,62 @@ ip_vpass_kernel(const __grid_constant__ IpParams P, const unsigned char* __restr
   o[2 * hw] = __ldg(norm + 512 + (swap_rb ? v0 : v2));
 }
 
+struct IpRotate {
+  int a[6];             // Pillow's affine_fixed coefficients a0..a5 (16.16) of Image.rotate on the fW x fH crop
+  int flip;             // 1: FLIP_LEFT_RIGHT of the crop before the rotation
+};
+
+struct IpRotateParams {
+  IpRotate img[IP_MAX_IMAGES];
+};
+
+// grid (column chunks, fH, M); block (m, output row blockIdx.y, output columns 256 * blockIdx.x + [0, 256)).  Output
+// pixel (x, y) of the rotated crop reads crop pixel ((a2 + y a1 + x a0) >> 16, (a5 + y a4 + x a3) >> 16) (0 outside the
+// crop), mirrored when flipped, i.e. resized pixel (x0 + column, y0 + row) (0 outside the resized image).  The host
+// checked that no intermediate leaves int32, as Pillow's int accumulation assumes.
+__global__ void __launch_bounds__(IP_THREADS)
+ip_vpass_aug_kernel(const __grid_constant__ IpParams P, const __grid_constant__ IpRotateParams Q,
+                    const unsigned char* __restrict__ ws, const float* __restrict__ norm, int swap_rb, int fH, int fW,
+                    float* __restrict__ out) {
+  const IpImage& d = P.img[blockIdx.z];
+  const IpRotate& q = Q.img[blockIdx.z];
+  const int y = blockIdx.y;
+  const int x = blockIdx.x * IP_THREADS + threadIdx.x;
+  if (x >= fW) return;
+  const int xs = (int)((q.a[2] + (long long)y * q.a[1] + (long long)x * q.a[0]) >> 16);
+  const int ys = (int)((q.a[5] + (long long)y * q.a[4] + (long long)x * q.a[3]) >> 16);
+  int v0 = 0, v1 = 0, v2 = 0;
+  if (xs >= 0 && xs < fW && ys >= 0 && ys < fH) {
+    const int R = d.y0 + ys, X = d.x0 + (q.flip ? fW - 1 - xs : xs);
+    if (R >= 0 && R < d.rH && X >= 0 && X < d.rW) {
+      const int lo = __ldg(d.vt + 2 * R) - d.r0;
+      const int n = min(__ldg(d.vt + 2 * R + 1), d.nr - lo);
+      const int col = X - d.c0;
+      if (lo >= 0 && col < d.nc) {
+        const long long plane = (long long)d.nr * d.nc;
+        const unsigned char* p = ws + d.ws + (long long)lo * d.nc + col;
+        const int* w = d.vt + 2 * d.rH + R;
+        int a0 = 1 << 21, a1 = 1 << 21, a2 = 1 << 21;
+        for (int k = 0; k < n; ++k) {
+          const int wk = __ldg(w + (long long)k * d.rH);
+          const unsigned char* r = p + (long long)k * d.nc;
+          a0 += wk * __ldg(r);
+          a1 += wk * __ldg(r + plane);
+          a2 += wk * __ldg(r + 2 * plane);
+        }
+        v0 = ip_clip8(a0);
+        v1 = ip_clip8(a1);
+        v2 = ip_clip8(a2);
+      }
+    }
+  }
+  const long long hw = (long long)fH * fW;
+  float* o = out + (long long)blockIdx.z * 3 * hw + (long long)y * fW + x;
+  o[0] = __ldg(norm + (swap_rb ? v2 : v0));
+  o[hw] = __ldg(norm + 256 + v1);
+  o[2 * hw] = __ldg(norm + 512 + (swap_rb ? v0 : v2));
+}
+
 // Pillow's precompute_coeffs (resample.c) for one output index: ksize and the tap window [first, first + count), in the
 // same float64 operations the host's table builder uses
 inline int ip_ksize(int in, int n) {
@@ -175,21 +236,16 @@ extern "C" size_t occ_prepare_images_workspace_bytes(const int* geom, int M, int
   return total;
 }
 
-extern "C" int occ_prepare_images(const unsigned char* frames, long long frame_bytes, const long long* offsets,
-                                  const int* geom, int M, int fH, int fW, const long long* tables, const float* norm,
-                                  int swap_rb, void* ws, size_t ws_bytes, float* out, cudaStream_t stream) {
-  OCC_REQUIRE(frames && offsets && geom && tables && norm && out && M >= 1 && M <= IP_MAX_IMAGES);
-  OCC_REQUIRE(fH >= 1 && fW >= 1 && (swap_rb == 0 || swap_rb == 1) && frame_bytes >= 0);
-  OCC_REQUIRE((long long)fH * fW <= (1LL << 31) && (long long)fH < 65536);
-  OCC_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 15) == 0);
-  IpParams P;  // 18 KB of kernel parameters (sm_90 takes up to 32 KB)
+// the descriptors of both entries' M images -> 0 or the entry's error code; *ws_need, *max_nr, *max_nc for the launch
+static int ip_setup(const char* fn, long long frame_bytes, const long long* offsets, const int* geom, int M, int fH,
+                    int fW, const long long* tables, IpParams* P, size_t* ws_need, int* max_nr, int* max_nc) {
   size_t ws_off = 0;
-  int max_nr = 0, max_nc = 0;
+  *max_nr = *max_nc = 0;
   for (int m = 0; m < M; ++m) {
-    IpImage& d = P.img[m];
+    IpImage& d = P->img[m];
     const int rc = ip_describe(geom + 6 * m, fH, fW, &d);
     if (rc != OCC_OK) {
-      if (rc == OCC_EINVAL) fprintf(stderr, "occ_b200: occ_prepare_images: bad geometry of image %d\n", m);
+      if (rc == OCC_EINVAL) fprintf(stderr, "occ_b200: %s: bad geometry of image %d\n", fn, m);
       return rc;
     }
     const int H = geom[6 * m];
@@ -202,9 +258,26 @@ extern "C" int occ_prepare_images(const unsigned char* frames, long long frame_b
     d.vt = reinterpret_cast<const int*>(tables[2 * m + 1]);
     d.ws = (long long)ws_off;
     ws_off += ip_align((size_t)3 * d.nr * d.nc);
-    max_nr = d.nr > max_nr ? d.nr : max_nr;
-    max_nc = d.nc > max_nc ? d.nc : max_nc;
+    *max_nr = d.nr > *max_nr ? d.nr : *max_nr;
+    *max_nc = d.nc > *max_nc ? d.nc : *max_nc;
   }
+  *ws_need = ws_off;
+  return OCC_OK;
+}
+
+extern "C" int occ_prepare_images(const unsigned char* frames, long long frame_bytes, const long long* offsets,
+                                  const int* geom, int M, int fH, int fW, const long long* tables, const float* norm,
+                                  int swap_rb, void* ws, size_t ws_bytes, float* out, cudaStream_t stream) {
+  OCC_REQUIRE(frames && offsets && geom && tables && norm && out && M >= 1 && M <= IP_MAX_IMAGES);
+  OCC_REQUIRE(fH >= 1 && fW >= 1 && (swap_rb == 0 || swap_rb == 1) && frame_bytes >= 0);
+  OCC_REQUIRE((long long)fH * fW <= (1LL << 31) && (long long)fH < 65536);
+  OCC_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 15) == 0);
+  IpParams P;  // 18 KB of kernel parameters (sm_90 takes up to 32 KB)
+  size_t ws_off = 0;
+  int max_nr = 0, max_nc = 0;
+  const int rc = ip_setup("occ_prepare_images", frame_bytes, offsets, geom, M, fH, fW, tables, &P, &ws_off, &max_nr,
+                          &max_nc);
+  if (rc != OCC_OK) return rc;
   OCC_REQUIRE(ws_bytes >= ws_off && (ws_off == 0 || ws));
   if (max_nr > 0) {
     const dim3 grid((unsigned)((max_nc + IP_THREADS - 1) / IP_THREADS), (unsigned)max_nr, (unsigned)M);
@@ -214,6 +287,50 @@ extern "C" int occ_prepare_images(const unsigned char* frames, long long frame_b
   const dim3 grid((unsigned)((fW + IP_THREADS - 1) / IP_THREADS), (unsigned)fH, (unsigned)M);
   ip_vpass_kernel<<<grid, IP_THREADS, 0, stream>>>(P, static_cast<const unsigned char*>(ws), norm, swap_rb, fH, fW,
                                                    out);
+  OCC_LAUNCH_CHECK();
+  return OCC_OK;
+}
+
+extern "C" int occ_prepare_images_aug(const unsigned char* frames, long long frame_bytes, const long long* offsets,
+                                      const int* geom, const int* aug, int M, int fH, int fW, const long long* tables,
+                                      const float* norm, int swap_rb, void* ws, size_t ws_bytes, float* out,
+                                      cudaStream_t stream) {
+  OCC_REQUIRE(frames && offsets && geom && aug && tables && norm && out && M >= 1 && M <= IP_MAX_IMAGES);
+  OCC_REQUIRE(fH >= 1 && fW >= 1 && (swap_rb == 0 || swap_rb == 1) && frame_bytes >= 0);
+  OCC_REQUIRE((long long)fH * fW <= (1LL << 31) && (long long)fH < 65536);
+  OCC_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 15) == 0);
+  for (int m = 0; m < M; ++m) {
+    const int* g = aug + 7 * m;
+    OCC_REQUIRE(g[0] == 0 || g[0] == 1);
+    // every intermediate of a + y * a1 + x * a0 at the crop's corners (hence everywhere inside) fits in int32
+    for (int c = 0; c < 2; ++c) {
+      const long long a0 = g[1 + 3 * c], a1 = g[2 + 3 * c], a2 = g[3 + 3 * c];
+      const long long lo = a2 + (a1 < 0 ? a1 * (fH - 1) : 0) + (a0 < 0 ? a0 * (fW - 1) : 0);
+      const long long hi = a2 + (a1 > 0 ? a1 * (fH - 1) : 0) + (a0 > 0 ? a0 * (fW - 1) : 0);
+      OCC_REQUIRE(lo >= INT32_MIN && hi <= INT32_MAX);
+    }
+  }
+  IpParams P;
+  size_t ws_off = 0;
+  int max_nr = 0, max_nc = 0;
+  const int rc = ip_setup("occ_prepare_images_aug", frame_bytes, offsets, geom, M, fH, fW, tables, &P, &ws_off,
+                          &max_nr, &max_nc);
+  if (rc != OCC_OK) return rc;
+  OCC_REQUIRE(ws_bytes >= ws_off && (ws_off == 0 || ws));
+  IpRotateParams R;  // 7 KB beside P's 18 KB of kernel parameters
+  for (int m = 0; m < M; ++m) {
+    const int* g = aug + 7 * m;
+    R.img[m].flip = g[0];
+    for (int k = 0; k < 6; ++k) R.img[m].a[k] = g[1 + k];
+  }
+  if (max_nr > 0) {
+    const dim3 grid((unsigned)((max_nc + IP_THREADS - 1) / IP_THREADS), (unsigned)max_nr, (unsigned)M);
+    ip_hpass_kernel<<<grid, IP_THREADS, 0, stream>>>(P, frames, static_cast<unsigned char*>(ws));
+    OCC_LAUNCH_CHECK();
+  }
+  const dim3 grid((unsigned)((fW + IP_THREADS - 1) / IP_THREADS), (unsigned)fH, (unsigned)M);
+  ip_vpass_aug_kernel<<<grid, IP_THREADS, 0, stream>>>(P, R, static_cast<const unsigned char*>(ws), norm, swap_rb, fH,
+                                                       fW, out);
   OCC_LAUNCH_CHECK();
   return OCC_OK;
 }

@@ -12,6 +12,11 @@ into the frames prepare_images takes; the loader then ships the JPEG bytes inste
 (pipelines.LoadMultiViewJpegBytes_OccFormer).  decode_png does the same for SemanticKITTI's PNG frames
 (csrc/png_decode.cu, pipelines.LoadMultiViewPngBytes_SemanticKitti).
 
+Training pipelines add per camera 'flip' and 'rotate' to img_aug (pipelines.LoadMultiViewImageFramesAug_*), which
+prepare_images then applies as Pillow's FLIP_LEFT_RIGHT and Image.rotate (rotate_coeffs); LoadLidarDepthPoints adds
+the LiDAR scan, from which lidar_depth_maps builds CreateDepthFromLiDAR's depth maps; camera_inputs does both for a
+training step.
+
 The host part here is table building: Pillow's bicubic coefficients per (source size, resized size) of an axis and the
 normalisation as a 3 x 256 table, both in float64 numpy, one operation at a time as x86-64 builds of Pillow and OpenCV
 compute them (no fused multiply-add).  ops.prepare_images caches them on the device.
@@ -90,6 +95,9 @@ def prepare_images(frames, img_aug):
         samples = list(frames)
     if len(samples) != len(img_aug) or not samples:
         raise ValueError(f"prepare_images: {len(samples)} samples of frames but {len(img_aug)} img_aug metas")
+    train = [("flip" in a) or ("rotate" in a) for a in img_aug]
+    if any(train) and not all(train):
+        raise ValueError("prepare_images: a batch mixes training-mode img_aug (flip / rotate) and test-mode img_aug")
     for s in samples:
         if s.dtype != torch.uint8 or s.dim() != 4 or s.shape[-1] != 3:
             raise ValueError(f"prepare_images: every sample must be uint8 (N, H, W, 3), got {s.dtype} "
@@ -112,15 +120,89 @@ def prepare_images(frames, img_aug):
         flat = frames.reshape(-1)
     else:
         flat = torch.cat([s.contiguous().reshape(-1) for s in samples])
-    offsets, geoms, off = [], [], 0
+    offsets, geoms, aug, off = [], [], [], 0
     for s, a in zip(samples, img_aug):
         H, W = int(s.shape[1]), int(s.shape[2])
-        for (rW, rH), crop in zip(a["resize_dims"], a["crop"]):
+        for c, ((rW, rH), crop) in enumerate(zip(a["resize_dims"], a["crop"])):
             offsets.append(off)
             geoms.append((H, W, int(rW), int(rH), int(crop[0]), int(crop[1])))
             off += H * W * 3
-    out = ops.prepare_images(flat, offsets, geoms, size, norm["mean"], norm["std"], norm["to_rgb"])
+            if train[0]:
+                flip = bool(a.get("flip", [False] * N)[c])
+                aug.append((int(flip),) + rotate_coeffs(a.get("rotate", [0.0] * N)[c], size[1], size[0]))
+    out = ops.prepare_images(flat, offsets, geoms, size, norm["mean"], norm["std"], norm["to_rgb"],
+                             aug if train[0] else None)
     return out.view(len(samples), N, 3, *size)
+
+
+def rotate_coeffs(angle, w, h):
+    """Pillow's Image.rotate(angle) (NEAREST, no expand, black fill) of a w x h image as the six 16.16 fixed-point
+    coefficients (a0, .., a5) of its affine_fixed gather: output (x, y) reads ((a2 + y a1 + x a0) >> 16,
+    (a5 + y a4 + x a3) >> 16), 0 outside.  Pillow copies at angle 0 and transposes at 180, and at 90 / 270 for a square
+    image: those take the coefficients of the same permutation.  Otherwise the matrix is Image.rotate's float64 one
+    about (w / 2, h / 2), and FIX(v) = floor(v * 65536 + 0.5) as in Pillow's Geometry.c."""
+    angle = angle % 360.0
+    one = 1 << 16
+    if angle == 0:
+        return (one, 0, 0, 0, one, 0)
+    if angle == 180:
+        return (-one, 0, (w - 1) << 16, 0, -one, (h - 1) << 16)
+    if angle == 90 and w == h:   # Transpose.ROTATE_90: out (x, y) = in (w - 1 - y, x)
+        return (0, -one, (w - 1) << 16, one, 0, 0)
+    if angle == 270 and w == h:  # Transpose.ROTATE_270: out (x, y) = in (y, h - 1 - x)
+        return (0, one, 0, -one, 0, (h - 1) << 16)
+    a = -math.radians(angle)
+    m = [round(math.cos(a), 15), round(math.sin(a), 15), 0.0, round(-math.sin(a), 15), round(math.cos(a), 15), 0.0]
+    cx, cy = w / 2.0, h / 2.0
+    m[2] = m[0] * -cx + m[1] * -cy + m[2] + cx
+    m[5] = m[3] * -cx + m[4] * -cy + m[5] + cy
+    # Pillow takes the fixed-point path while the far corner maps inside +-32768 (check_fixed); past that it would
+    # interpolate in float64, which this gather does not restate
+    if not (abs(w * m[0] + h * m[1] + m[2]) < 32768.0 and abs(w * m[3] + h * m[4] + m[5]) < 32768.0):
+        raise ValueError(f"rotate_coeffs: a {w} x {h} image is past Pillow's fixed-point rotation")
+
+    def fix(v):
+        return math.floor(v * 65536.0 + 0.5)
+    return (fix(m[0]), fix(m[1]), fix(m[2] + m[1] * 0.5 + m[0] * 0.5), fix(m[3]), fix(m[4]),
+            fix(m[5] + m[4] * 0.5 + m[3] * 0.5))
+
+
+def lidar_depth_maps(points, img_inputs, img_aug):
+    """CreateDepthFromLiDAR's gt_depths on the GPU (csrc/lidar_depth.cu), bit for bit as a loader worker computes them:
+    points, B scans of float32 (P_b, 3) (host or CUDA); img_inputs, the collated tuple (trans, intrins, post_rots,
+    post_trans at [2:6], CUDA); img_aug, B metas with 'lidar_inv_rots' (pipelines.LoadLidarDepthPoints) and
+    'input_size' -> float32 (B, N, fH, fW).  The scans travel in one pinned host buffer and one host-to-device copy."""
+    if len(points) != len(img_aug) or not img_aug:
+        raise ValueError(f"lidar_depth_maps: {len(points)} scans but {len(img_aug)} img_aug metas")
+    trans, intrins, post_rots, post_trans = img_inputs[2:6]
+    dev = trans.device
+    B, N = trans.shape[:2]
+    size = [int(v) for v in img_aug[0]["input_size"]]
+    if any([int(v) for v in a["input_size"]] != size for a in img_aug):
+        raise ValueError("lidar_depth_maps: every sample of a batch needs the same input_size")
+    pts = [torch.as_tensor(p, dtype=torch.float32).reshape(-1, 3) for p in points]
+    offsets = np.cumsum([0] + [len(p) for p in pts]).tolist()
+    if all(p.is_cuda for p in pts):
+        flat = torch.cat(pts).contiguous()
+    else:
+        flat, _ = _stage([p.cpu().contiguous().numpy().view(np.uint8).reshape(-1) for p in pts])
+        flat = flat.view(torch.float32).view(-1, 3)
+    inv_rots = torch.stack([torch.as_tensor(a["lidar_inv_rots"], dtype=torch.float32) for a in img_aug]).to(dev)
+    return ops.lidar_depth(flat, offsets, inv_rots.contiguous(), trans.float().contiguous(),
+                           intrins.float().contiguous(), post_rots.float().contiguous(),
+                           post_trans.float().contiguous(), size)
+
+
+def camera_inputs(img_inputs, img_metas):
+    """The reference training pipeline's collated img_inputs on the GPU, from those of LoadMultiViewImageFramesAug_* +
+    LoadLidarDepthPoints: img_inputs[0] the uint8 frames (prepare_images), the gt_depths placeholder (the slot before
+    sensor2sensors: 6 of the loaders' 8-tuple, 7 once an occupancy annotation transform has added bda_rot) replaced by
+    lidar_depth_maps, every other element passed through.  img_metas: B dicts carrying 'img_aug'."""
+    img_aug = [m["img_aug"] for m in img_metas]
+    imgs = prepare_images(img_inputs[0], img_aug)
+    depths = lidar_depth_maps([a["lidar_points"] for a in img_aug], img_inputs, img_aug)
+    k = len(img_inputs) - 2
+    return (imgs,) + tuple(img_inputs[1:k]) + (depths,) + tuple(img_inputs[k + 1:])
 
 
 def decode_jpeg(files, names=None, seq_bits=ops.JPEG_SEQ_BITS, sync_rounds=ops.JPEG_SYNC_ROUNDS):

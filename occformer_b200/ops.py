@@ -1004,10 +1004,11 @@ def _prep_table(dev, in_size, out_size):
     return t
 
 
-def prepare_images(frames, offsets, geoms, input_size, mean, std, to_rgb):
+def prepare_images(frames, offsets, geoms, input_size, mean, std, to_rgb, aug=None):
     """M camera images from uint8 BGR frames (occ_prepare_images): frames a flat uint8 CUDA buffer, image m the H x W x 3
-    bytes at offsets[m], geoms[m] = (H, W, rW, rH, x0, y0) -> float32 (M, 3, fH, fW).  The coefficient and normalisation
-    tables are built once per geometry and config and kept on the device; no synchronisation."""
+    bytes at offsets[m], geoms[m] = (H, W, rW, rH, x0, y0) -> float32 (M, 3, fH, fW).  aug: None, or per image
+    (flip, a0, .., a5), the training loaders' flip and rotation (occ_prepare_images_aug).  The coefficient and
+    normalisation tables are built once per geometry and config and kept on the device; no synchronisation."""
     M = len(geoms)
     fH, fW = (int(v) for v in input_size)
     dev = frames.device
@@ -1028,8 +1029,24 @@ def prepare_images(frames, offsets, geoms, input_size, mean, std, to_rgb):
         ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
         _prep_ws[key] = ws
     out = torch.empty((M, 3, fH, fW), dtype=torch.float32, device=dev)
-    _call("occ_prepare_images", frames, frames.numel(), (ctypes.c_longlong * M)(*offsets), geom, M, fH, fW,
-          (ctypes.c_longlong * (2 * M))(*tables), norm, int(bool(to_rgb)), ws, ws.numel(), out)
+    head = [frames, frames.numel(), (ctypes.c_longlong * M)(*offsets), geom]
+    tail = [M, fH, fW, (ctypes.c_longlong * (2 * M))(*tables), norm, int(bool(to_rgb)), ws, ws.numel(), out]
+    if aug is None:
+        _call("occ_prepare_images", *head, *tail)
+    else:
+        _call("occ_prepare_images_aug", *head, (ctypes.c_int * (7 * M))(*[int(v) for a in aug for v in a]), *tail)
+    return out
+
+
+def lidar_depth(pts, offsets, inv_rots, trans, intrins, post_rots, post_trans, input_size):
+    """Depth maps of B samples x N cameras (occ_lidar_depth): pts (n, 3) fp32 CUDA, sample b's points at rows
+    [offsets[b], offsets[b + 1]); inv_rots, trans, intrins (3 x 3 or 4 x 4), post_rots, post_trans fp32 CUDA (B, N, ...)
+    -> float32 (B, N, fH, fW); no synchronisation."""
+    B, N = trans.shape[:2]
+    fH, fW = (int(v) for v in input_size)
+    out = torch.empty((B, N, fH, fW), dtype=torch.float32, device=trans.device)
+    _call("occ_lidar_depth", pts if pts.numel() else None, (ctypes.c_longlong * (B + 1))(*offsets), B, N, inv_rots,
+          trans, intrins, int(intrins.shape[-1]), post_rots, post_trans, fH, fW, out)
     return out
 
 

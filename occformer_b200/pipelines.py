@@ -1,6 +1,8 @@
 """Loader transforms that leave the occupancy ground truth (occformer_b200.targets), the camera images' resize, crop and
 normalisation (occformer_b200.image_prep, the LoadMultiViewImageFrames_* transforms) or also the JPEG decoding
-(LoadMultiViewJpegBytes_OccFormer) to the GPU.  LoadSemKittiVoxelFiles, at the end of this file, hands SemanticKITTI's
+(LoadMultiViewJpegBytes_OccFormer) to the GPU.  In training pipelines, the LoadMultiViewImageFramesAug_* transforms
+also leave the flip and rotation, and LoadLidarDepthPoints the depth maps of CreateDepthFromLiDAR, to the GPU
+(image_prep.camera_inputs).  LoadSemKittiVoxelFiles, at the end of this file, hands SemanticKITTI's
 voxel files to the GPU in place of the preprocessed labels.
 
     LoadNuscOccupancyPoints          = LoadNuscOccupancyAnnotations          P/datasets/pipelines/loading_nusc_occ.py:13-120
@@ -116,14 +118,21 @@ class LoadNuscPanopticOccupancyPoints(_OccupancyPoints):
 
 # ---------------------------------------------------------------------------------------------- camera images
 class _ImageFrames:
-    """the shared part of the two image transforms: test-mode sample_augmentation (loading_nusc_imgs.py:84-95), the
-    post-homography in the reference's float32 torch arithmetic (:39-53), and the frame decode"""
+    """the shared part of the image transforms: sample_augmentation (loading_nusc_imgs.py:72-96) in test mode, or with
+    the training-mode draws when the class sets ``training``, the post-homography in the reference's float32 torch
+    arithmetic (:34-53), and the frame decode.  A transform serves one mode and refuses the other."""
+
+    training = False
 
     def __init__(self, data_config, is_train=False, img_norm_cfg=None):
-        if is_train:
-            raise ValueError(f"{type(self).__name__}: is_train=True is not supported: the package has no training step, "
-                             "and CreateDepthFromLiDAR reads the image size from the normalised images; keep the "
-                             "reference transform for training pipelines")
+        if is_train and not self.training:
+            raise ValueError(f"{type(self).__name__}: is_train=True is not supported by this test-mode transform; "
+                             "training pipelines take LoadMultiViewImageFramesAug_OccFormer / "
+                             "LoadMultiViewImageFramesAug_SemanticKitti (with LoadLidarDepthPoints in place of "
+                             "CreateDepthFromLiDAR), or keep the reference transform")
+        if self.training and not is_train:
+            raise ValueError(f"{type(self).__name__}: is_train=False: this is the training-mode transform; test "
+                             "pipelines take LoadMultiViewImageFrames_OccFormer / LoadMultiViewImageFrames_SemanticKitti")
         from .image_prep import norm_config
         self.is_train, self.data_config, self.img_norm_cfg = is_train, data_config, img_norm_cfg
         self.norm = norm_config(img_norm_cfg)
@@ -138,12 +147,40 @@ class _ImageFrames:
         crop_w = int(max(0, newW - fW) / 2)
         return resize, resize_dims, (crop_w, crop_h, crop_w + fW, crop_h + fH)
 
+    def train_augmentation(self, H, W):
+        """training-mode sample_augmentation: five numpy draws in the reference's order (resize, crop_h, crop_w, flip,
+        rotate; no flip draw when data_config['flip'] is falsy) -> (resize, resize_dims, crop, flip, rotate)"""
+        cfg = self.data_config
+        fH, fW = cfg["input_size"]
+        resize = float(fW) / float(W)
+        resize += np.random.uniform(*cfg["resize"])
+        resize_dims = (int(W * resize), int(H * resize))
+        newW, newH = resize_dims
+        crop_h = int((1 - np.random.uniform(*cfg["crop_h"])) * newH) - fH
+        crop_w = int(np.random.uniform(0, max(0, newW - fW)))
+        flip = cfg["flip"] and np.random.choice([0, 1])
+        rotate = np.random.uniform(*cfg["rot"])
+        return resize, resize_dims, (crop_w, crop_h, crop_w + fW, crop_h + fH), flip, rotate
+
+    def choose_cams(self):
+        """the camera names of a sample: in training mode Ncams of them drawn without replacement when Ncams is fewer"""
+        cams = self.data_config["cams"]
+        if self.training and self.data_config["Ncams"] < len(cams):
+            return np.random.choice(cams, self.data_config["Ncams"], replace=False)
+        return cams
+
     @staticmethod
-    def post_homography(resize, crop):
-        """(post_rot (3, 3), post_tran (3,)) of img_transform with flip False and rotate 0"""
+    def post_homography(resize, crop, flip=False, rotate=0):
+        """(post_rot (3, 3), post_tran (3,)) of img_transform"""
         post_rot2 = torch.eye(2) * resize
         post_tran2 = torch.zeros(2) - torch.Tensor(crop[:2])
-        A = torch.Tensor([[np.cos(0.0), np.sin(0.0)], [-np.sin(0.0), np.cos(0.0)]])
+        if flip:
+            A = torch.Tensor([[-1, 0], [0, 1]])
+            b = torch.Tensor([crop[2] - crop[0], 0])
+            post_rot2 = A.matmul(post_rot2)
+            post_tran2 = A.matmul(post_tran2) + b
+        h = rotate / 180 * np.pi
+        A = torch.Tensor([[np.cos(h), np.sin(h)], [-np.sin(h), np.cos(h)]])
         b = torch.Tensor([crop[2] - crop[0], crop[3] - crop[1]]) / 2
         b = A.matmul(-b) + b
         post_rot2 = A.matmul(post_rot2)
@@ -165,13 +202,19 @@ class _ImageFrames:
         return img
 
     def camera(self, img):
-        """one decoded frame -> (resize_dims, crop, post_rot, post_tran)"""
-        resize, resize_dims, crop = self.sample_augmentation(img.shape[0], img.shape[1])
-        return (resize_dims, crop) + self.post_homography(resize, crop)
+        """one decoded frame -> (resize_dims, crop, flip, rotate, post_rot, post_tran)"""
+        if self.training:
+            resize, resize_dims, crop, flip, rotate = self.train_augmentation(img.shape[0], img.shape[1])
+        else:
+            (resize, resize_dims, crop), flip, rotate = self.sample_augmentation(img.shape[0], img.shape[1]), False, 0
+        return (resize_dims, crop, flip, rotate) + self.post_homography(resize, crop, flip, rotate)
 
-    def img_aug(self, dims, crops):
-        return dict(resize_dims=[list(d) for d in dims], crop=[list(c) for c in crops],
-                    input_size=list(self.data_config["input_size"]), **self.norm)
+    def img_aug(self, dims, crops, flips=(), rotates=()):
+        aug = dict(resize_dims=[list(d) for d in dims], crop=[list(c) for c in crops],
+                   input_size=list(self.data_config["input_size"]), **self.norm)
+        if self.training:
+            aug.update(flip=[bool(f) for f in flips], rotate=[float(r) for r in rotates])
+        return aug
 
 
 @PIPELINES.register_module()
@@ -183,15 +226,16 @@ class LoadMultiViewImageFrames_OccFormer(_ImageFrames):
     results['canvas'] (the cropped uint8 images, read only by a commented-out visualisation) is not produced."""
 
     def __call__(self, results):
-        cam_names = self.data_config["cams"]
+        cam_names = self.choose_cams()
         results["cam_names"] = cam_names
-        frames, rots, trans, intrins, post_rots, post_trans, sensor2sensors, dims, crops = ([] for _ in range(9))
+        frames, rots, trans, intrins, post_rots, post_trans, sensor2sensors, dims, crops, flips, rotates = (
+            [] for _ in range(11))
         for cam_name in cam_names:
             cam_data = results["curr"]["cams"][cam_name]
             img = self.decode(cam_data["data_path"])
             intrin = torch.Tensor(cam_data["cam_intrinsic"])
             sensor2lidar = torch.tensor(results["lidar2cam_dic"][cam_name]).inverse().float()
-            resize_dims, crop, post_rot, post_tran = self.camera(img)
+            resize_dims, crop, flip, rotate, post_rot, post_tran = self.camera(img)
             frames.append(torch.from_numpy(img))
             intrins.append(intrin)
             rots.append(sensor2lidar[:3, :3])
@@ -201,12 +245,14 @@ class LoadMultiViewImageFrames_OccFormer(_ImageFrames):
             sensor2sensors.append(sensor2lidar)
             dims.append(resize_dims)
             crops.append(crop)
+            flips.append(flip)
+            rotates.append(rotate)
         if len({tuple(f.shape) for f in frames}) != 1:
-            raise ValueError("LoadMultiViewImageFrames_OccFormer: the cameras of a sample need one frame size")
+            raise ValueError(f"{type(self).__name__}: the cameras of a sample need one frame size")
         gt_depths = [torch.zeros(1) for _ in cam_names]
         results["img_inputs"] = tuple(torch.stack(x) for x in (frames, rots, trans, intrins, post_rots, post_trans,
                                                                 gt_depths, sensor2sensors))
-        results["img_aug"] = self.img_aug(dims, crops)
+        results["img_aug"] = self.img_aug(dims, crops, flips, rotates)
         return results
 
 
@@ -221,14 +267,65 @@ class LoadMultiViewImageFrames_SemanticKitti(_ImageFrames):
         assert len(img_filenames) == 1
         img = self.decode(img_filenames[0])
         results["raw_img"] = img
-        resize_dims, crop, post_rot, post_tran = self.camera(img)
+        resize_dims, crop, flip, rotate, post_rot, post_tran = self.camera(img)
         intrin = torch.Tensor(results["cam_intrinsic"][0])
         lidar2cam = torch.Tensor(results["lidar2cam"][0])
         cam2lidar = lidar2cam.inverse()
         res = [torch.from_numpy(img), cam2lidar[:3, :3], cam2lidar[:3, 3], intrin, post_rot, post_tran, torch.zeros(1),
                cam2lidar]
         results["img_inputs"] = tuple(x[None] for x in res)
-        results["img_aug"] = self.img_aug([resize_dims], [crop])
+        results["img_aug"] = self.img_aug([resize_dims], [crop], [flip], [rotate])
+        return results
+
+
+@PIPELINES.register_module()
+class LoadMultiViewImageFramesAug_OccFormer(LoadMultiViewImageFrames_OccFormer):
+    """LoadMultiViewImageFromFiles_OccFormer (loading_nusc_imgs.py:10-179) in training mode (is_train=True is required),
+    leaving the resize, crop, flip, rotation and normalisation to the GPU (image_prep.camera_inputs).  The same numpy
+    draws in the same order as the reference (choose_cams when Ncams < len(cams), then per camera resize, crop_h,
+    crop_w, flip when data_config['flip'], rotate) and the same img_inputs[1:]; img_inputs[0] is the decoded uint8
+    (N, H, W, 3) BGR frames and results['img_aug'] also carries each camera's 'flip' and 'rotate'."""
+
+    training = True
+
+
+@PIPELINES.register_module()
+class LoadMultiViewImageFramesAug_SemanticKitti(LoadMultiViewImageFrames_SemanticKitti):
+    """LoadMultiViewImageFromFiles_SemanticKitti (loading_kitti_imgs.py:12-146) in training mode (is_train=True is
+    required), leaving the resize, crop, flip, rotation and normalisation to the GPU: the reference's draws and
+    img_inputs[1:], the decoded uint8 (1, H, W, 3) BGR frame in img_inputs[0], and 'flip' / 'rotate' in
+    results['img_aug']."""
+
+    training = True
+
+
+@PIPELINES.register_module()
+class LoadLidarDepthPoints:
+    """CreateDepthFromLiDAR (P/datasets/pipelines/lidar2depth.py:8-87) leaving the projection to the GPU: reads the same
+    scan (nuScenes: pts_filename as (-1, 5) float32 rows; KITTI: the velodyne .bin of the camera frame under data_root,
+    as (-1, 4) rows), keeps x, y, z, and computes rots.inverse() of img_inputs[1] here, in CPU fp32 torch as the
+    reference does (a device inverse would give other bits).  Both go into results['img_aug'] ('lidar_points',
+    'lidar_inv_rots'); img_inputs keeps its 8-tuple layout with the gt_depths placeholder, which
+    image_prep.camera_inputs fills on the GPU.  Makes no random draws."""
+
+    def __init__(self, data_root=None, dataset="kitti"):
+        if dataset not in ("kitti", "nusc"):
+            raise ValueError(f"LoadLidarDepthPoints: dataset must be 'kitti' or 'nusc', got {dataset!r}")
+        self.data_root, self.dataset = data_root, dataset
+
+    def scan_path(self, results):
+        if self.dataset == "nusc":
+            return results["pts_filename"]
+        seq_id, _, filename = results["img_filename"][0].split("/")[-3:]
+        return os.path.join(self.data_root, "data_velodyne/velodyne/sequences", seq_id, "velodyne",
+                            filename.replace(".png", ".bin"))
+
+    def __call__(self, results):
+        cols = 4 if self.dataset == "kitti" else 5
+        pts = np.fromfile(self.scan_path(results), dtype=np.float32).reshape(-1, cols)[:, :3]
+        inv_rots = results["img_inputs"][1].inverse()
+        results["img_aug"] = dict(results["img_aug"], lidar_points=torch.from_numpy(np.ascontiguousarray(pts)),
+                                  lidar_inv_rots=inv_rots)
         return results
 
 
