@@ -47,7 +47,7 @@ struct GemmParams {
                   // (zero-initialised by the host) through TMA reduce-add; no bias / act / stats in the kernel
   int act;        // 0 none, 1 relu, 2 gelu(erf), 3 swish
   int split_out;  // write the result in the S32 split format (the consumer is another tensor-core contraction)
-  int passes;     // tensor-core passes per 32-k block (occ_common.cuh: mma_passes)
+  int passes;     // tensor-core passes per 32-k block (occ_common.cuh: mma_passes): picks the PASSES instantiation
   // conv mode
   int conv;
   int Cin, KX, KY, KZ, dil, stride;
@@ -112,7 +112,9 @@ constexpr int acc_stage_bytes() { return 2 * 64 * acc_pitch<BN>() * 4; }
 // so warp w of the warpgroup holds the 32 consecutive tile rows 128cg + 32w .. +31 (16 of each chain) and stages them
 // chunk by chunk through its own TMA-store buffer: no fp32 staging block, which leaves room for a 4-deep ring.
 // No split-K.
-template <int BN, int STAGES, bool LEAN, int MT = 1>
+// PASSES: tensor-core passes per 32-k block (3 = fp32-faithful, 1 = single-pass bf16), fixed at compile time so that a
+// k-block's wgmmas form one straight-line batch behind a single wgmma_fence.
+template <int BN, int STAGES, bool LEAN, int MT, int PASSES>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ GemmParams p) {
@@ -238,6 +240,10 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     int stage = 0;
     uint32_t phase = 0;
     int cur_b = -1;
+    // A k-block that never arrives makes the warp leave both loops before any named barrier and trap after them: a trap
+    // reachable inside the loops would cap ptxas's register allocation at the launch bound (168), below the
+    // accumulators and epilogue of the 256-row tiles (occ_ptx.cuh: mbar_wait).
+    bool timed_out = false;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int n_tile = (tile / f_splits) % num_n_tiles;
       const int m_tile = tile / (f_splits * num_n_tiles);
@@ -253,17 +259,17 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
           for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.f;
         int prev_stage = -1;
         for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
+          if (!mbar_wait_bounded(&full_bar[stage], phase)) { timed_out = true; break; }
           const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
           const uint64_t bdesc = make_sw128_desc(sa + A_BYTES, 1024, 16);
           wgmma_fence();
           // one S32 row block = 32 k values: hi*hi + lo*hi + hi*lo, six K=16 wgmmas stepping 32 bytes inside the row
           if constexpr (MT == 1) {
-            wgmma_bf16x3_ss<BN>(acc[0], make_sw128_desc(sa + cg * (64 * 128), 1024, 16), bdesc, 1u, p.passes);
+            wgmma_bf16x3_ss<BN, PASSES>(acc[0], make_sw128_desc(sa + cg * (64 * 128), 1024, 16), bdesc, 1u);
           } else {
             const uint32_t a0 = sa + cg * (128 * 128);
-            wgmma_bf16x3_ss2<BN>(acc[0], acc[MT - 1], make_sw128_desc(a0, 2048, 16), make_sw128_desc(a0 + 1024, 2048, 16),
-                                 bdesc, 1u, p.passes);
+            wgmma_bf16x3_ss2<BN, PASSES>(acc[0], acc[MT - 1], make_sw128_desc(a0, 2048, 16),
+                                         make_sw128_desc(a0 + 1024, 2048, 16), bdesc, 1u);
           }
           wgmma_commit();
           wgmma_wait<1>();  // the previous k-block's wgmmas have finished reading their stage
@@ -274,6 +280,7 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         wgmma_wait<0>();
 #pragma unroll
         for (int h = 0; h < MT; ++h) wgmma_fence_regs(acc[h]);
+        if (timed_out) break;
         if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
         if constexpr (MT == 1) {
           // fragment -> row-major staging block of this warpgroup (the previous tile's epilogue finished reading it)
@@ -500,6 +507,7 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         }
       }
     }
+    if (timed_out) __trap();
     if (f_stats) {
       asm volatile("bar.sync 1, 256;" ::: "memory");
       if (cur_b >= 0) {
@@ -577,19 +585,27 @@ static int launch_gn_stats(const float* x, double* stats, int B, int rows_per_sa
 // ring depth of an instantiation: as deep as the shared memory allows (MT = 2 has no fp32 staging block)
 constexpr int gemm_stages(int bn, int mt) { return mt == 2 ? 4 : bn <= 32 ? 8 : bn <= 64 ? 6 : bn <= 96 ? 4 : 3; }
 
-template <int BN, bool LEAN = false, int MT = 1>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmParams& p,
-                       int num_tiles, cudaStream_t stream) {
+template <int BN, bool LEAN, int MT, int PASSES>
+static int launch_gemm_passes(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmParams& p,
+                              int num_tiles, cudaStream_t stream) {
   constexpr int STAGES = gemm_stages(BN, MT);
   constexpr size_t smem = (size_t)STAGES * (MT * A_STAGE_BYTES + BN * BK * 4) + 1024 /*align*/ + CTRL_BYTES + EPI_BYTES +
                           (MT == 1 ? acc_stage_bytes<BN>() : 0);
   static_assert(smem <= 227 * 1024, "shared memory budget");
-  OCC_ENSURE_SMEM((gemm_bf16x3_kernel<BN, STAGES, LEAN, MT>), smem);
+  OCC_ENSURE_SMEM((gemm_bf16x3_kernel<BN, STAGES, LEAN, MT, PASSES>), smem);
   int grid = num_tiles < sm_count() ? num_tiles : sm_count();
   if (grid < 1) grid = 1;
-  gemm_bf16x3_kernel<BN, STAGES, LEAN, MT><<<grid, GEMM_THREADS, smem, stream>>>(tmA, tmB, tmC, p);
+  gemm_bf16x3_kernel<BN, STAGES, LEAN, MT, PASSES><<<grid, GEMM_THREADS, smem, stream>>>(tmA, tmB, tmC, p);
   OCC_LAUNCH_CHECK();
   return OCC_OK;
+}
+
+// p.passes (mma_passes() at the call) selects the three-pass or the single-pass instantiation
+template <int BN, bool LEAN = false, int MT = 1>
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmParams& p,
+                       int num_tiles, cudaStream_t stream) {
+  if (p.passes == 1) return launch_gemm_passes<BN, LEAN, MT, 1>(tmA, tmB, tmC, p, num_tiles, stream);
+  return launch_gemm_passes<BN, LEAN, MT, 3>(tmA, tmB, tmC, p, num_tiles, stream);
 }
 
 // N-tile: 96-wide tiles for the 192-channel neck / head matrices (N = 192, 576: no padded columns), else 32 / 64 / 128

@@ -91,7 +91,7 @@ __device__ __forceinline__ void ntf_layernorm(float (&acc)[E / 2], const float* 
   }
 }
 
-template <int E>
+template <int E, int PASSES>  // PASSES: tensor-core passes per 32-k block, fixed so that each wgmma batch is one straight line
 __global__ void __launch_bounds__(NTF_THREADS, 1)
 neck_tail_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmWo,
                  const __grid_constant__ CUtensorMap tmW1, const __grid_constant__ CUtensorMap tmW2,
@@ -189,8 +189,8 @@ neck_tail_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         wait_slot(2 * kb);
         wait_slot(2 * kb + 1);
         wgmma_fence();
-        wgmma_bf16x3_ss<E>(acc, make_sw128_desc(slot_addr(2 * kb) + cg * (64 * 128), 1024, 16),
-                           make_sw128_desc(slot_addr(2 * kb + 1), 1024, 16), kb != 0, p.passes);
+        wgmma_bf16x3_ss<E, PASSES>(acc, make_sw128_desc(slot_addr(2 * kb) + cg * (64 * 128), 1024, 16),
+                                   make_sw128_desc(slot_addr(2 * kb + 1), 1024, 16), kb != 0);
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(acc);
@@ -238,8 +238,8 @@ neck_tail_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         wgmma_fence();
 #pragma unroll
         for (int kb = 0; kb < KB; ++kb)
-          wgmma_bf16x3_ss<32>(h, make_sw128_desc(xs_addr + kb * (64 * 128), 1024, 16),
-                              make_sw128_desc(w1 + kb * 4096, 1024, 16), kb != 0, p.passes);
+          wgmma_bf16x3_ss<32, PASSES>(h, make_sw128_desc(xs_addr + kb * (64 * 128), 1024, 16),
+                                      make_sw128_desc(w1 + kb * 4096, 1024, 16), kb != 0);
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(h);
@@ -255,7 +255,7 @@ neck_tail_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
           wgmma_rs<E, 0>(acc, ah[hh], bdesc + 2 * hh, 1u);
-          if (p.passes == 3) {
+          if constexpr (PASSES == 3) {
             wgmma_rs<E, 0>(acc, al[hh], bdesc + 2 * hh, 1u);
             wgmma_rs<E, 0>(acc, ah[hh], bdesc + 2 * (2 + hh), 1u);
           }
@@ -326,12 +326,16 @@ static int launch_neck_tail(const float* att, const float* wo, const float* w1, 
   if (!rc) rc = make_tmap_f32(&tmW2, w2, 2, w2dims, fstrides, ebox, nullptr);
   if (rc) return rc;
   const size_t smem = NeckTailShape<E>::smem(p.F);
-  OCC_ENSURE_SMEM(neck_tail_kernel<E>, smem);
   int grid = sm_count();
   if (grid > p.n_tiles) grid = p.n_tiles;
-  neck_tail_kernel<E><<<grid, NTF_THREADS, smem, stream>>>(tmA, tmWo, tmW1, tmW2, p);
-  OCC_LAUNCH_CHECK();
-  return OCC_OK;
+  auto launch = [&](auto passes) {
+    constexpr int P = decltype(passes)::value;
+    OCC_ENSURE_SMEM((neck_tail_kernel<E, P>), smem);
+    neck_tail_kernel<E, P><<<grid, NTF_THREADS, smem, stream>>>(tmA, tmWo, tmW1, tmW2, p);
+    OCC_LAUNCH_CHECK();
+    return OCC_OK;
+  };
+  return p.passes == 1 ? launch(std::integral_constant<int, 1>{}) : launch(std::integral_constant<int, 3>{});
 }
 
 }  // namespace occ

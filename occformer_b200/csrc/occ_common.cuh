@@ -110,7 +110,8 @@ __device__ __forceinline__ int ordered_logit(float x) {
 
 // Tensor-core passes per 32-k operand block: 3 = fp32-faithful (hi*hi + lo*hi + hi*lo, the default and the only mode the
 // parity gate covers), 1 = single-pass bf16 (hi*hi only; occ_set_mma_passes, csrc/config.cu).  Host-side setting, read by
-// every launcher at launch time and handed to the kernel as an argument.
+// every launcher at launch time and handed to the kernel as an argument (the GEMM / conv launcher picks the kernel
+// instantiation compiled for that pass count).
 int mma_passes();
 
 // fp32 tensor map, rank <= 5, 128-byte swizzle, zero OOB fill.  dims/box/estr innermost first;

@@ -56,9 +56,9 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// Time-bounded wait: a mis-programmed pipeline traps (-> launch error) after ~4 s instead of hanging the GPU box
-// (try_wait may suspend the thread for a while, so the bound is taken from %globaltimer, not from the spin count).
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+// Time-bounded wait: false once ~4 s have passed without the phase completing (try_wait may suspend the thread for a
+// while, so the bound is taken from %globaltimer, not from the spin count).
+__device__ __forceinline__ bool mbar_wait_bounded(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   unsigned long long t0 = 0;
   while (!mbar_try_wait(bar, parity)) {
@@ -66,9 +66,16 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       unsigned long long t;
       asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
       if (t0 == 0) t0 = t;
-      else if (t - t0 > 4000000000ull) __trap();
+      else if (t - t0 > 4000000000ull) return false;
     }
   }
+  return true;
+}
+// A mis-programmed pipeline traps (-> launch error) instead of hanging the GPU box.  (A trap reachable inside a loop
+// caps ptxas's register allocation at the launch bound, whatever setmaxnreg grants: a register-heavy wgmma main loop
+// waits with mbar_wait_bounded and traps after leaving its loops.)
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+  if (!mbar_wait_bounded(bar, parity)) __trap();
 }
 
 // ------------------------------------------------------------------ fences
@@ -334,16 +341,33 @@ __device__ __forceinline__ void wgmma_bf16x3_ss(float (&d)[N / 2], uint64_t ades
   }
 }
 
+// The same with the pass count fixed at compile time (PASSES = 3 or 1): the 6 or 2 wgmmas form one straight-line batch
+// (a run-time test between them splits the batch, and ptxas re-arms the warpgroup before every piece).  The GEMM / conv,
+// Swin, window-attention and neck-tail kernels use this form; the decoder's kernels still pass the count at run time.
+template <int N, int PASSES>
+__device__ __forceinline__ void wgmma_bf16x3_ss(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t acc0) {
+  static_assert(PASSES == 1 || PASSES == 3, "passes per 32-k block");
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    wgmma_ss<N>(d, adesc + 2 * h, bdesc + 2 * h, h ? 1u : acc0);  // hi * hi
+    if constexpr (PASSES == 3) {
+      wgmma_ss<N>(d, adesc + 2 * (2 + h), bdesc + 2 * h, 1u);     // lo * hi
+      wgmma_ss<N>(d, adesc + 2 * h, bdesc + 2 * (2 + h), 1u);     // hi * lo
+    }
+  }
+}
+
 // The same for two M = 64 chains (two A tiles, two accumulators) on one B tile: the wgmmas of the two chains alternate,
 // so each chain's dependent wgmma overlaps with the other's; every chain keeps the accumulation order of the above.
-template <int N>
+template <int N, int PASSES>
 __device__ __forceinline__ void wgmma_bf16x3_ss2(float (&d0)[N / 2], float (&d1)[N / 2], uint64_t adesc0, uint64_t adesc1,
-                                                 uint64_t bdesc, uint32_t acc0, int passes = 3) {
+                                                 uint64_t bdesc, uint32_t acc0) {
+  static_assert(PASSES == 1 || PASSES == 3, "passes per 32-k block");
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     wgmma_ss<N>(d0, adesc0 + 2 * h, bdesc + 2 * h, h ? 1u : acc0);
     wgmma_ss<N>(d1, adesc1 + 2 * h, bdesc + 2 * h, h ? 1u : acc0);
-    if (passes == 3) {
+    if constexpr (PASSES == 3) {
       wgmma_ss<N>(d0, adesc0 + 2 * (2 + h), bdesc + 2 * h, 1u);
       wgmma_ss<N>(d1, adesc1 + 2 * (2 + h), bdesc + 2 * h, 1u);
       wgmma_ss<N>(d0, adesc0 + 2 * h, bdesc + 2 * (2 + h), 1u);

@@ -33,6 +33,7 @@ constexpr int SF_OFF_QB = SF_OFF_BIAS + WA_BIAS_BYTES;                  // 22323
 constexpr int SF_OFF_BAR = SF_OFF_QB + 384;                             // 223616
 constexpr int SF_SMEM = SF_OFF_BAR + 2 * SF_NSLOT * 8 + 1024;           // 224768 <= 232448 (227 KB)
 
+template <int PASSES>  // tensor-core passes per 32-k block, fixed so that each wgmma batch is one straight line
 __global__ void __launch_bounds__(SF_THREADS, 1)
 swin_qkv_attn_kernel(const __grid_constant__ CUtensorMap tmap_tok /*window-layout tokens (npairs*128, 128) S32, box 32 x 128*/,
                      const float* __restrict__ wqkv /*(384, 128) S32,
@@ -114,8 +115,8 @@ swin_qkv_attn_kernel(const __grid_constant__ CUtensorMap tmap_tok /*window-layou
       for (int kb = 0; kb < SF_KB; ++kb) {
         mbar_wait(&a_full[slot], par);
         wgmma_fence();
-        wgmma_bf16x3_ss<96>(d, make_sw128_desc(smem_u32(sa + (size_t)slot * SF_SLOT) + half * (64 * 128), 1024, 16),
-                            wdesc0 + (uint64_t)(kb * ((96 * 128) >> 4)), kb != 0, g.passes);
+        wgmma_bf16x3_ss<96, PASSES>(d, make_sw128_desc(smem_u32(sa + (size_t)slot * SF_SLOT) + half * (64 * 128), 1024, 16),
+                                    wdesc0 + (uint64_t)(kb * ((96 * 128) >> 4)), kb != 0);
         wgmma_commit();
         wgmma_wait<1>();
         if (prev >= 0 && lane == 0) mbar_arrive(&a_empty[prev]);
@@ -173,7 +174,7 @@ swin_qkv_attn_kernel(const __grid_constant__ CUtensorMap tmap_tok /*window-layou
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         wgmma_rs<64, 0>(sc, qh[hh], kdesc + 2 * hh, hh != 0);                 // hi * hi
-        if (g.passes == 3) {
+        if constexpr (PASSES == 3) {
           wgmma_rs<64, 0>(sc, ql[hh], kdesc + 2 * hh, 1u);                    // lo * hi
           wgmma_rs<64, 0>(sc, qh[hh], kdesc + 2 * (2 + hh), 1u);              // hi * lo
         }
@@ -182,7 +183,7 @@ swin_qkv_attn_kernel(const __grid_constant__ CUtensorMap tmap_tok /*window-layou
       wgmma_wait<0>();
       wgmma_fence_regs(sc);
       float o[32], sum[2];
-      wa_softmax_pv(sc, sb, t, diff, vdesc, g.passes, o, sum);
+      wa_softmax_pv<PASSES>(sc, sb, t, diff, vdesc, o, sum);
       wa_store_rows(o, sum, row, t, out, g.C, h);
     }
   }
@@ -207,7 +208,6 @@ extern "C" int occ_swin_qkv_attention(const float* tokn, const float* wqkv, cons
   const WinGeom g = make_win_geom(B, X, Y, Z, C, heads, shift);
   OCC_REQUIRE(g.nwin < (1ll << 31));
   static_assert(SF_SMEM <= 227 * 1024, "shared memory budget");
-  OCC_ENSURE_SMEM(swin_qkv_attn_kernel, SF_SMEM);
   const long long npairs = (g.nwin + 1) / 2;
   long long groups = sm_count() / heads;
   if (groups > npairs) groups = npairs;
@@ -219,7 +219,12 @@ extern "C" int occ_swin_qkv_attention(const float* tokn, const float* wqkv, cons
     const uint32_t box[2] = {32, 128};
     OCC_REQUIRE(make_tmap_f32(&tm, tokn, 2, dims, strides, box, nullptr) == OCC_OK);
   }
-  swin_qkv_attn_kernel<<<(int)(groups * heads), SF_THREADS, SF_SMEM, stream>>>(tm, wqkv, bqkv, bias_pad, out, g);
-  OCC_LAUNCH_CHECK();
-  return OCC_OK;
+  auto launch = [&](auto passes) {
+    constexpr int P = decltype(passes)::value;
+    OCC_ENSURE_SMEM(swin_qkv_attn_kernel<P>, SF_SMEM);
+    swin_qkv_attn_kernel<P><<<(int)(groups * heads), SF_THREADS, SF_SMEM, stream>>>(tm, wqkv, bqkv, bias_pad, out, g);
+    OCC_LAUNCH_CHECK();
+    return OCC_OK;
+  };
+  return g.passes == 1 ? launch(std::integral_constant<int, 1>{}) : launch(std::integral_constant<int, 3>{});
 }

@@ -54,6 +54,7 @@ __device__ __forceinline__ float smf_gelu(float x) {
   return x * phi;
 }
 
+template <int PASSES>  // tensor-core passes per 32-k block, fixed so that each wgmma batch is one straight line
 __global__ void __launch_bounds__(SMF_THREADS, 1)
 swin_mlp_fused_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmWp,
                       const __grid_constant__ CUtensorMap tmW1, const __grid_constant__ CUtensorMap tmW2,
@@ -135,7 +136,7 @@ swin_mlp_fused_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         for (int hh = 0; hh < 2; ++hh) {
           const int ks = 2 * kb + hh;
           wgmma_rs<128, 0>(d, ah[ks], bdesc + 2 * hh, (kb | hh) ? 1u : acc0);
-          if (p.passes == 3) {
+          if constexpr (PASSES == 3) {
             wgmma_rs<128, 0>(d, al[ks], bdesc + 2 * hh, 1u);
             wgmma_rs<128, 0>(d, ah[ks], bdesc + 2 * (2 + hh), 1u);
           }
@@ -157,8 +158,8 @@ swin_mlp_fused_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         wait_slot(2 * kb);
         wait_slot(2 * kb + 1);
         wgmma_fence();
-        wgmma_bf16x3_ss<128>(acc, make_sw128_desc(slot_addr(2 * kb) + cg * (64 * 128), 1024, 16),
-                             make_sw128_desc(slot_addr(2 * kb + 1), 1024, 16), kb != 0, p.passes);
+        wgmma_bf16x3_ss<128, PASSES>(acc, make_sw128_desc(slot_addr(2 * kb) + cg * (64 * 128), 1024, 16),
+                                     make_sw128_desc(slot_addr(2 * kb + 1), 1024, 16), kb != 0);
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(acc);
@@ -275,10 +276,14 @@ extern "C" int occ_swin_proj_ffn(const float* att, const float* tok, const float
   p.n_tiles = (int)((M + 127) / 128);
   const size_t smem = (size_t)SMF_SLOTS * SMF_SLOT + 2 * SMF_STASH + 5 * SMF_C * sizeof(float) + 2 * SMF_SLOTS * 8 +
                       1024 /*align*/;
-  OCC_ENSURE_SMEM(swin_mlp_fused_kernel, smem);
   int grid = sm_count();
   if (grid > p.n_tiles) grid = p.n_tiles;
-  swin_mlp_fused_kernel<<<grid, SMF_THREADS, smem, stream>>>(tmA, tmWp, tmW1, tmW2, p);
-  OCC_LAUNCH_CHECK();
-  return OCC_OK;
+  auto launch = [&](auto passes) {
+    constexpr int P = decltype(passes)::value;
+    OCC_ENSURE_SMEM(swin_mlp_fused_kernel<P>, smem);
+    swin_mlp_fused_kernel<P><<<grid, SMF_THREADS, smem, stream>>>(tmA, tmWp, tmW1, tmW2, p);
+    OCC_LAUNCH_CHECK();
+    return OCC_OK;
+  };
+  return p.passes == 1 ? launch(std::integral_constant<int, 1>{}) : launch(std::integral_constant<int, 3>{});
 }

@@ -30,6 +30,7 @@
 
 namespace occ {
 
+template <int PASSES>  // tensor-core passes per 32-k block, fixed so that each wgmma batch is one straight line
 __global__ void __launch_bounds__(WA_THREADS, 1)
 window_attn_tc_kernel(const float* __restrict__ qkv, const float* __restrict__ qkv_bias,
                       const float* __restrict__ bias_pad /*(heads, 2404)*/, float* __restrict__ out, const WinGeom g) {
@@ -151,12 +152,12 @@ window_attn_tc_kernel(const float* __restrict__ qkv, const float* __restrict__ q
 #pragma unroll
       for (int j = 0; j < 32; ++j) sc[j] = 0.f;
       wgmma_fence();
-      wgmma_bf16x3_ss<64>(sc, make_sw128_desc(base, 1024, 16), make_sw128_desc(base + WA_TILE, 1024, 16), 0u, g.passes);
+      wgmma_bf16x3_ss<64, PASSES>(sc, make_sw128_desc(base, 1024, 16), make_sw128_desc(base + WA_TILE, 1024, 16), 0u);
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_fence_regs(sc);
       float o[32], sum[2];
-      wa_softmax_pv(sc, sb, t, diff, make_sw128_desc(base + 2 * WA_TILE, 1024, 1024), g.passes, o, sum);
+      wa_softmax_pv<PASSES>(sc, sb, t, diff, make_sw128_desc(base + 2 * WA_TILE, 1024, 1024), o, sum);
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_bar[s]);
       wa_store_rows(o, sum, row, t, out, g.C, h);
@@ -182,13 +183,17 @@ extern "C" int occ_window_attention(const float* qkv, const float* qkv_bias, con
   OCC_REQUIRE(g.nwin < (1ll << 31));
   const size_t smem = (size_t)WA_STAGES * WA_STAGE_BYTES + WA_BIAS_BYTES + 1024 /*align*/ + 256 /*barriers*/;
   static_assert((size_t)WA_STAGES * WA_STAGE_BYTES + WA_BIAS_BYTES + 1024 + 256 <= 227 * 1024, "shared memory budget");
-  OCC_ENSURE_SMEM(window_attn_tc_kernel, smem);
   const long long npairs = (g.nwin + 1) / 2;
   OCC_REQUIRE(heads <= sm_count());
   long long groups = sm_count() / heads;  // CTA groups of `heads` CTAs, one head each
   if (groups > npairs) groups = npairs;
   const int grid = (int)(groups * heads);
-  window_attn_tc_kernel<<<grid, WA_THREADS, smem, stream>>>(qkv, qkv_bias, bias_pad, out, g);
-  OCC_LAUNCH_CHECK();
-  return OCC_OK;
+  auto launch = [&](auto passes) {
+    constexpr int P = decltype(passes)::value;
+    OCC_ENSURE_SMEM(window_attn_tc_kernel<P>, smem);
+    window_attn_tc_kernel<P><<<grid, WA_THREADS, smem, stream>>>(qkv, qkv_bias, bias_pad, out, g);
+    OCC_LAUNCH_CHECK();
+    return OCC_OK;
+  };
+  return g.passes == 1 ? launch(std::integral_constant<int, 1>{}) : launch(std::integral_constant<int, 3>{});
 }

@@ -96,8 +96,9 @@ __device__ __forceinline__ uint64_t window_same_mask(const WinGeom& g, int wx, i
 // diff[r]: keys outside the row's shift-mask region (additive -100, as the reference).  The probabilities are split into
 // hi / lo register A fragments and multiplied with the V tile (vdesc: MN-major SWIZZLE_128B, 64 key rows of
 // [hi | lo] of the head dim = N 64): o[:, :32] + o[:, 32:] = unnormalised P V; sum[r] = softmax denominators.
+template <int PASSES>
 __device__ __forceinline__ void wa_softmax_pv(float (&s)[32], const float* __restrict__ sb, const int (&t)[2],
-                                              const uint64_t (&diff)[2], uint64_t vdesc, int passes, float (&o)[32],
+                                              const uint64_t (&diff)[2], uint64_t vdesc, float (&o)[32],
                                               float (&sum)[2]) {
   const int q = threadIdx.x & 3;
   const float sl2 = 0.17677669529663687f * 1.4426950408889634f;  // 32^-0.5 * log2 e: scores live in the log2 domain
@@ -141,7 +142,7 @@ __device__ __forceinline__ void wa_softmax_pv(float (&s)[32], const float* __res
 #pragma unroll
   for (int kk = 0; kk < 4; ++kk) {  // 16 keys per wgmma = two 8-key (1024 B) atoms of V rows
     wgmma_rs<64, 1>(o, ph[kk], vdesc + (uint64_t)(kk * 128), kk != 0);           // P_hi [V_hi | V_lo]
-    if (passes == 3) wgmma_rs<64, 1>(o, pl[kk], vdesc + (uint64_t)(kk * 128), 1u);  // P_lo [V_hi | V_lo]
+    if constexpr (PASSES == 3) wgmma_rs<64, 1>(o, pl[kk], vdesc + (uint64_t)(kk * 128), 1u);  // P_lo [V_hi | V_lo]
   }
   wgmma_commit();
   wgmma_wait<0>();
