@@ -500,6 +500,25 @@ int occ_lidarseg_occupancy(const float* pts, int ld, const long long* offsets /*
 int occ_semkitti_labels(const unsigned char* label, const unsigned char* invalid, int B, long long nvox,
                         const int* lut, int lut_size, int* bad, long long* out, occ_stream_t stream);
 
+/* The training-mode SemanticKITTI ground truth (csrc/semkitti_labels.cu): occ_semkitti_labels' volume through
+ *   LoadSemKittiAnnotation(is_train=True) / voxel_transform   P/datasets/pipelines/loading_kitti_occ.py:34-53,55-117
+ *   custom_rotate_3d                                          P/datasets/pipelines/loading_nusc_occ.py:206-225
+ * bit for bit: .astype(np.uint8), then, when the sample's rotate flag is set, Image.rotate(angle, NEAREST,
+ * fillcolor=255) of every z slice (a 256 x 256 mode-"L" image, rows = x, columns = y), then [:, :, ::-1] when flip_dz,
+ * [:, ::-1] when flip_dy, [::-1] when flip_dx, then .long().  The volume is SemanticKITTI's 256 x 256 x 32.
+ *   label, invalid  as occ_semkitti_labels with nvox = 2^21; label 16-byte aligned, invalid 4-byte aligned
+ *   aug             device int32 (B, 10), 4-byte aligned: flip_dx, flip_dy, flip_dz, rotate (each 0 / nonzero), then
+ *                   a0..a5, the 16.16 coefficients of occ_prepare_images_aug (occformer_b200.image_prep.rotate_coeffs of
+ *                   (angle, 256, 256), Pillow's copy and transposes included): output slice pixel (y, x) reads
+ *                   (x', y') = ((a5 + x a4 + y a3) >> 16, (a2 + x a1 + y a0) >> 16), 255 outside the slice; the host
+ *                   sets rotate only when not np.isclose(angle, 0), as the reference decides; ignored when rotate = 0
+ *   lut             as occ_semkitti_labels; its values must lie in [0, 255] (the reference's uint8 cast)
+ *   out             (B, 256, 256, 32) int64, 16-byte aligned, overwritten
+ * A label >= lut_size adds to bad[b] (B device ints, ACCUMULATED) once per voxel of the source volume, whether or not
+ * the rotation reads it, and is written as 255.  1 <= B <= 65536.  One launch per call, no host synchronisation. */
+int occ_semkitti_labels_aug(const unsigned char* label, const unsigned char* invalid, int B, const int* aug,
+                            const int* lut, int lut_size, int* bad, long long* out, occ_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------------------
  * Camera images from the decoded frames (csrc/image_prep.cu): steps 2-4 of the test loaders' image side,
  *   LoadMultiViewImageFromFiles_OccFormer     P/datasets/pipelines/loading_nusc_imgs.py:34-62,181-195

@@ -125,17 +125,14 @@ class OccupancyFormer(nn.Module):
         placeholder: the JPEG files in each 'img_aug' are decoded on the GPU first (image_prep.decode_jpeg); so is
         LoadMultiViewPngBytes_SemanticKitti's (B, 1, 0) one, whose 'img_aug' carries PNG files (image_prep.decode_png)."""
         imgs = img[0]
-        if torch.is_tensor(imgs) and imgs.dtype == torch.uint8 and imgs.dim() == 3 and imgs.shape[-1] == 0:
+        if image_prep.is_file_placeholder(imgs):
             augs = [m.get("img_aug", {}) for m in img_metas] if img_metas is not None else []
-            kind = next((k for k in ("png", "jpeg") if augs and all(k in a for a in augs)), None)
-            if kind is None:
+            imgs = image_prep.decode_files(augs)
+            if imgs is None:
                 raise ValueError("OccupancyFormer: the empty image placeholder needs each sample's 'img_aug' meta with "
                                  "its 'jpeg' files, which LoadMultiViewJpegBytes_OccFormer produces, or its 'png' files, "
                                  "which LoadMultiViewPngBytes_SemanticKitti produces; add 'img_aug' to Collect3D's "
                                  "meta_keys")
-            names = [a.get(kind + "_files") for a in augs]
-            decode = image_prep.decode_png if kind == "png" else image_prep.decode_jpeg
-            imgs = decode([a[kind] for a in augs], None if None in names else names)
         if (imgs.dtype if torch.is_tensor(imgs) else imgs[0].dtype) == torch.uint8:
             if img_metas is None or any("img_aug" not in m for m in img_metas):
                 raise ValueError("OccupancyFormer: uint8 camera frames need each sample's 'img_aug' meta, which the "
@@ -209,7 +206,9 @@ class OccupancyFormer(nn.Module):
         img_metas[0] -> int64 (B, X, Y, Z): semantic labels for Mask2FormerNuscOccHead, panoptic ids for
         Mask2FormerNuscPanopticOccHead.  Reads one invalid-point count back to the host (ValueError if nonzero).
         Mask2FormerOccHead (SemanticKITTI): points_occ is unused; every sample's img_metas carry the 'semkitti_voxels' of
-        LoadSemKittiVoxelFiles -> int64 (B, 256, 256, 32) from those files (targets.semantic_kitti_occupancy)."""
+        LoadSemKittiVoxelFiles -> int64 (B, 256, 256, 32) from those files (targets.semantic_kitti_occupancy); those of
+        the training transform LoadSemKittiVoxelFilesAug also carry its 'augment', which gives the augmented volume of
+        LoadSemKittiAnnotation(is_train=True) (semantic_kitti_occupancy(..., augment=))."""
         head = self.pts_bbox_head
         if isinstance(head, Mask2FormerNuscPanopticOccHead):
             build = targets.panoptic_occupancy
@@ -219,8 +218,13 @@ class OccupancyFormer(nn.Module):
             vox = [m["semkitti_voxels"] for m in img_metas]
             if any(v["learning_map"] != vox[0]["learning_map"] for v in vox[1:]):
                 raise ValueError("occupancy_targets: every sample of a batch needs the same learning map")
+            aug = {"augment" in v for v in vox}
+            if len(aug) != 1:
+                raise ValueError("occupancy_targets: a batch mixes the voxel files of LoadSemKittiVoxelFiles and of "
+                                 "LoadSemKittiVoxelFilesAug")
+            kw = dict(augment=[v["augment"] for v in vox]) if aug == {True} else {}
             return targets.semantic_kitti_occupancy([v["label"] for v in vox], [v["invalid"] for v in vox],
-                                                    vox[0]["learning_map"], names=[v["files"] for v in vox])
+                                                    vox[0]["learning_map"], names=[v["files"] for v in vox], **kw)
         else:
             raise NotImplementedError(f"occupancy_targets: {type(head).__name__} scores against preprocessed voxel labels "
                                       "(SemanticKITTI), not a LiDAR point scan; pass gt_occ, or the voxel files of "

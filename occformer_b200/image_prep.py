@@ -193,13 +193,38 @@ def lidar_depth_maps(points, img_inputs, img_aug):
                            post_trans.float().contiguous(), size)
 
 
+def is_file_placeholder(imgs):
+    """the empty uint8 (B, N, 0) img_inputs[0] of the byte transforms (pipelines.LoadMultiView*Bytes*)"""
+    return torch.is_tensor(imgs) and imgs.dtype == torch.uint8 and imgs.dim() == 3 and imgs.shape[-1] == 0
+
+
+def decode_files(img_aug):
+    """the frames of the files the byte transforms put into img_aug: 'png' files in every meta (decode_png), else
+    'jpeg' files in every meta (decode_jpeg), named by 'png_files' / 'jpeg_files' -> decoded frames; None when the metas
+    carry neither"""
+    kind = next((k for k in ("png", "jpeg") if img_aug and all(k in a for a in img_aug)), None)
+    if kind is None:
+        return None
+    names = [a.get(kind + "_files") for a in img_aug]
+    decode = decode_png if kind == "png" else decode_jpeg
+    return decode([a[kind] for a in img_aug], None if None in names else names)
+
+
 def camera_inputs(img_inputs, img_metas):
-    """The reference training pipeline's collated img_inputs on the GPU, from those of LoadMultiViewImageFramesAug_* +
-    LoadLidarDepthPoints: img_inputs[0] the uint8 frames (prepare_images), the gt_depths placeholder (the slot before
-    sensor2sensors: 6 of the loaders' 8-tuple, 7 once an occupancy annotation transform has added bda_rot) replaced by
-    lidar_depth_maps, every other element passed through.  img_metas: B dicts carrying 'img_aug'."""
+    """The reference training pipeline's collated img_inputs on the GPU, from those of LoadMultiViewImageFramesAug_* (or
+    LoadMultiViewJpegBytesAug_OccFormer / LoadMultiViewPngBytesAug_SemanticKitti) + LoadLidarDepthPoints: img_inputs[0]
+    the uint8 frames (prepare_images), or the byte transforms' empty placeholder, whose files are decoded first
+    (decode_files); the gt_depths placeholder (the slot before sensor2sensors: 6 of the loaders' 8-tuple, 7 once an
+    occupancy annotation transform has added bda_rot) replaced by lidar_depth_maps; every other element passed through.
+    img_metas: B dicts carrying 'img_aug'."""
     img_aug = [m["img_aug"] for m in img_metas]
-    imgs = prepare_images(img_inputs[0], img_aug)
+    frames = img_inputs[0]
+    if is_file_placeholder(frames):
+        frames = decode_files(img_aug)
+        if frames is None:
+            raise ValueError("camera_inputs: the empty image placeholder needs each sample's 'img_aug' meta with its "
+                             "'jpeg' or 'png' files, which the byte transforms produce")
+    imgs = prepare_images(frames, img_aug)
     depths = lidar_depth_maps([a["lidar_points"] for a in img_aug], img_inputs, img_aug)
     k = len(img_inputs) - 2
     return (imgs,) + tuple(img_inputs[1:k]) + (depths,) + tuple(img_inputs[k + 1:])

@@ -988,6 +988,21 @@ def semkitti_labels(label, invalid, B, nvox, lut):
     return out, bad
 
 
+def semkitti_labels_aug(label, invalid, B, aug, lut):
+    """the training-mode SemanticKITTI ground truth of B samples (occ_semkitti_labels_aug): label / invalid / lut as
+    semkitti_labels with nvox = 256 * 256 * 32, aug int32 CUDA (B, 10) rows (flip_dx, flip_dy, flip_dz, rotate,
+    a0..a5) -> (int64 (B, 256, 256, 32) volume, int32 (B,) count of labels past the LUT per sample); no
+    synchronisation."""
+    if label.numel() != B * 2 * 256 * 256 * 32 or invalid.numel() != B * 256 * 256 * 4 or aug.numel() != B * 10:
+        raise RuntimeError(f"occformer_b200: occ_semkitti_labels_aug: B = {B} needs {B * 2 << 21} label bytes, "
+                           f"{B << 18} invalid bytes and {B * 10} aug values, got {label.numel()}, {invalid.numel()}, "
+                           f"{aug.numel()}")
+    out = torch.empty((B, 256, 256, 32), dtype=torch.int64, device=label.device)
+    bad = torch.zeros(B, dtype=torch.int32, device=label.device)
+    _call("occ_semkitti_labels_aug", label, invalid, B, aug, lut, lut.numel(), bad, out)
+    return out, bad
+
+
 # ----------------------------------------------------------------------------------------------- camera images
 _prep_tables = {}  # (device, source size, resized size) -> int32 resample table of one axis (image_prep.resample_table)
 _prep_norms = {}   # (device, mean, std, to_rgb) -> float32 (3, 256) normalisation table

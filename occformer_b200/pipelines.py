@@ -2,8 +2,10 @@
 normalisation (occformer_b200.image_prep, the LoadMultiViewImageFrames_* transforms) or also the JPEG decoding
 (LoadMultiViewJpegBytes_OccFormer) to the GPU.  In training pipelines, the LoadMultiViewImageFramesAug_* transforms
 also leave the flip and rotation, and LoadLidarDepthPoints the depth maps of CreateDepthFromLiDAR, to the GPU
-(image_prep.camera_inputs).  LoadSemKittiVoxelFiles, at the end of this file, hands SemanticKITTI's
-voxel files to the GPU in place of the preprocessed labels.
+(image_prep.camera_inputs), and the byte transforms' training twins (LoadMultiViewJpegBytesAug_OccFormer,
+LoadMultiViewPngBytesAug_SemanticKitti) also the decode.  LoadSemKittiVoxelFiles, at the end of this file, hands
+SemanticKITTI's voxel files to the GPU in place of the preprocessed labels, and LoadSemKittiVoxelFilesAug does so in
+training pipelines with LoadSemKittiAnnotation's augmentation.
 
     LoadNuscOccupancyPoints          = LoadNuscOccupancyAnnotations          P/datasets/pipelines/loading_nusc_occ.py:13-120
     LoadNuscPanopticOccupancyPoints  = LoadNuscPanopticOccupancyAnnotations  P/datasets/pipelines/loading_nusc_panoptic_occ.py:32-145
@@ -203,10 +205,14 @@ class _ImageFrames:
 
     def camera(self, img):
         """one decoded frame -> (resize_dims, crop, flip, rotate, post_rot, post_tran)"""
+        return self.camera_size(img.shape[0], img.shape[1])
+
+    def camera_size(self, H, W):
+        """one camera of an H x W frame -> (resize_dims, crop, flip, rotate, post_rot, post_tran)"""
         if self.training:
-            resize, resize_dims, crop, flip, rotate = self.train_augmentation(img.shape[0], img.shape[1])
+            resize, resize_dims, crop, flip, rotate = self.train_augmentation(H, W)
         else:
-            (resize, resize_dims, crop), flip, rotate = self.sample_augmentation(img.shape[0], img.shape[1]), False, 0
+            (resize, resize_dims, crop), flip, rotate = self.sample_augmentation(H, W), False, 0
         return (resize_dims, crop, flip, rotate) + self.post_homography(resize, crop, flip, rotate)
 
     def img_aug(self, dims, crops, flips=(), rotates=()):
@@ -340,10 +346,10 @@ class LoadMultiViewJpegBytes_OccFormer(LoadMultiViewImageFrames_OccFormer):
 
     def __call__(self, results):
         from .jpeg import JpegError, frame_size
-        cam_names = self.data_config["cams"]
+        cam_names = self.choose_cams()
         results["cam_names"] = cam_names
-        files, paths, rots, trans, intrins, post_rots, post_trans, sensor2sensors, dims, crops, sizes = (
-            [] for _ in range(11))
+        files, paths, rots, trans, intrins, post_rots, post_trans, sensor2sensors, dims, crops, sizes, flips, rotates = (
+            [] for _ in range(13))
         for cam_name in cam_names:
             cam_data = results["curr"]["cams"][cam_name]
             path = cam_data["data_path"]
@@ -355,8 +361,7 @@ class LoadMultiViewJpegBytes_OccFormer(LoadMultiViewImageFrames_OccFormer):
                 raise ValueError(f"{path}: {e}") from None
             intrin = torch.Tensor(cam_data["cam_intrinsic"])
             sensor2lidar = torch.tensor(results["lidar2cam_dic"][cam_name]).inverse().float()
-            resize, resize_dims, crop = self.sample_augmentation(H, W)
-            post_rot, post_tran = self.post_homography(resize, crop)
+            resize_dims, crop, flip, rotate, post_rot, post_tran = self.camera_size(H, W)
             files.append(data)
             paths.append(path)
             sizes.append((H, W))
@@ -368,12 +373,14 @@ class LoadMultiViewJpegBytes_OccFormer(LoadMultiViewImageFrames_OccFormer):
             sensor2sensors.append(sensor2lidar)
             dims.append(resize_dims)
             crops.append(crop)
+            flips.append(flip)
+            rotates.append(rotate)
         if len(set(sizes)) != 1:
-            raise ValueError("LoadMultiViewJpegBytes_OccFormer: the cameras of a sample need one frame size")
+            raise ValueError(f"{type(self).__name__}: the cameras of a sample need one frame size")
         gt_depths = [torch.zeros(1) for _ in cam_names]
         results["img_inputs"] = (torch.zeros((len(cam_names), 0), dtype=torch.uint8),) + tuple(
             torch.stack(x) for x in (rots, trans, intrins, post_rots, post_trans, gt_depths, sensor2sensors))
-        results["img_aug"] = dict(self.img_aug(dims, crops), jpeg=files, jpeg_files=paths)
+        results["img_aug"] = dict(self.img_aug(dims, crops, flips, rotates), jpeg=files, jpeg_files=paths)
         return results
 
 
@@ -400,15 +407,35 @@ class LoadMultiViewPngBytes_SemanticKitti(LoadMultiViewImageFrames_SemanticKitti
             H, W = frame_size(data)
         except PngError as e:
             raise ValueError(f"{path}: {e}") from None
-        resize, resize_dims, crop = self.sample_augmentation(H, W)
-        post_rot, post_tran = self.post_homography(resize, crop)
+        resize_dims, crop, flip, rotate, post_rot, post_tran = self.camera_size(H, W)
         intrin = torch.Tensor(results["cam_intrinsic"][0])
         lidar2cam = torch.Tensor(results["lidar2cam"][0])
         cam2lidar = lidar2cam.inverse()
         res = [cam2lidar[:3, :3], cam2lidar[:3, 3], intrin, post_rot, post_tran, torch.zeros(1), cam2lidar]
         results["img_inputs"] = (torch.zeros((1, 0), dtype=torch.uint8),) + tuple(x[None] for x in res)
-        results["img_aug"] = dict(self.img_aug([resize_dims], [crop]), png=[data], png_files=[path])
+        results["img_aug"] = dict(self.img_aug([resize_dims], [crop], [flip], [rotate]), png=[data], png_files=[path])
         return results
+
+
+@PIPELINES.register_module()
+class LoadMultiViewJpegBytesAug_OccFormer(LoadMultiViewJpegBytes_OccFormer):
+    """LoadMultiViewImageFramesAug_OccFormer without the decode (is_train=True is required): the reference's training
+    draws (choose_cams when Ncams < len(cams), then per camera resize, crop_h, crop_w, flip when data_config['flip'],
+    rotate) with the frame size from each file's SOF header, the same img_inputs[1:] and img_aug ('flip' / 'rotate'
+    included), plus the files as LoadMultiViewJpegBytes_OccFormer adds them.  image_prep.camera_inputs decodes them on
+    the GPU first."""
+
+    training = True
+
+
+@PIPELINES.register_module()
+class LoadMultiViewPngBytesAug_SemanticKitti(LoadMultiViewPngBytes_SemanticKitti):
+    """LoadMultiViewImageFramesAug_SemanticKitti without the decode (is_train=True is required): the reference's
+    training draws with the frame size from the IHDR chunk, the same img_inputs[1:] and img_aug ('flip' / 'rotate'
+    included), plus the file as LoadMultiViewPngBytes_SemanticKitti adds it; no raw_img.  image_prep.camera_inputs
+    decodes it on the GPU first."""
+
+    training = True
 
 
 # ---------------------------------------------------------------------------------------------- SemanticKITTI labels
@@ -431,20 +458,97 @@ class LoadSemKittiVoxelFiles:
             raise ValueError("LoadSemKittiVoxelFiles: is_train=True is not supported: the transform hands no gt_occ to "
                              "LoadSemKittiAnnotation, whose training path needs it for the augmentation; keep the "
                              "preprocessed labels for training pipelines")
-        import yaml
-        with open(data_info_path, "r") as f:
-            self.learning_map = yaml.safe_load(f)["learning_map"]
+        self.learning_map = _learning_map(data_info_path)
         self.data_root, self.data_info_path = data_root, data_info_path
 
     def __call__(self, results):
-        from .targets import SEMKITTI_INVALID_BYTES, SEMKITTI_LABEL_BYTES
-        base = os.path.join(self.data_root, "dataset", "sequences", results["sequence"], "voxels", results["frame_id"])
-        files, data = [base + ".label", base + ".invalid"], []
-        for path, size in zip(files, (SEMKITTI_LABEL_BYTES, SEMKITTI_INVALID_BYTES)):
-            with open(path, "rb") as f:
-                data.append(f.read())
-            if len(data[-1]) != size:
-                raise ValueError(f"{path}: a SemanticKITTI voxel file of {size} bytes is needed, got {len(data[-1])}")
-        results["semkitti_voxels"] = dict(label=data[0], invalid=data[1], files=files, learning_map=self.learning_map)
+        results["semkitti_voxels"] = _voxel_files(self.data_root, results, self.learning_map)
         results["gt_occ"] = None
+        return results
+
+
+def _learning_map(data_info_path):
+    import yaml
+    with open(data_info_path, "r") as f:
+        return yaml.safe_load(f)["learning_map"]
+
+
+def _voxel_files(data_root, results, learning_map):
+    """dataset/sequences/{sequence}/voxels/{frame_id}.label and .invalid under data_root -> the 'semkitti_voxels' dict
+    (label=, invalid= (the files' bytes), files= (their paths), learning_map=); ValueError for a wrong size"""
+    from .targets import SEMKITTI_INVALID_BYTES, SEMKITTI_LABEL_BYTES
+    base = os.path.join(data_root, "dataset", "sequences", results["sequence"], "voxels", results["frame_id"])
+    files, data = [base + ".label", base + ".invalid"], []
+    for path, size in zip(files, (SEMKITTI_LABEL_BYTES, SEMKITTI_INVALID_BYTES)):
+        with open(path, "rb") as f:
+            data.append(f.read())
+        if len(data[-1]) != size:
+            raise ValueError(f"{path}: a SemanticKITTI voxel file of {size} bytes is needed, got {len(data[-1])}")
+    return dict(label=data[0], invalid=data[1], files=files, learning_map=learning_map)
+
+
+def semkitti_bda_matrix(rotate_deg, flip_dx, flip_dy, flip_dz, point_cloud_range):
+    """the 4x4 float32 bda_mat of the reference's SemanticKITTI voxel_transform (loading_kitti_occ.py:55-95), in its
+    torch arithmetic and product order: ((denorm @ flip) @ rot) @ norm, about the centre of point_cloud_range (taken
+    through torch.tensor, as LoadSemKittiAnnotation.__init__ takes it)"""
+    pcr = torch.tensor(point_cloud_range)
+    center = (pcr[:3] + pcr[3:]) / 2
+    norm, denorm = torch.eye(4), torch.eye(4)
+    norm[:3, -1] = -center
+    denorm[:3, -1] = center
+    a = torch.tensor(rotate_deg / 180 * np.pi)
+    s, c = torch.sin(a), torch.cos(a)
+    rot = torch.Tensor([[c, -s, 0, 0], [s, c, 0, 0], [0, 0, 1, 0], [0, 0, 0, 1]])
+    flip = torch.eye(4)
+    for axis, on in enumerate((flip_dx, flip_dy, flip_dz)):
+        if on:
+            f = torch.eye(4)
+            f[axis, axis] = -1
+            flip = flip @ f
+    return denorm @ flip @ rot @ norm
+
+
+@PIPELINES.register_module()
+class LoadSemKittiVoxelFilesAug:
+    """LoadSemKittiAnnotation(is_train=True) (P/datasets/pipelines/loading_kitti_occ.py:8-53) from the dataset's own voxel
+    files, leaving the volume and its augmentation to the GPU; it takes LoadSemKittiAnnotation's place in a training
+    pipeline.  The same kwargs (bda_aug_conf, is_train, point_cloud_range) plus LoadSemKittiVoxelFiles' data_root and
+    data_info_path.  It makes the reference's five numpy draws in its order (rotate, scale, flip_dx, flip_dy, flip_dz;
+    only the rotation and the flips are used), inserts the reference's 4x4 bda_mat (semkitti_bda_matrix) into
+    img_inputs as the reference does (the 9-tuple), and puts the files, the learning map and
+    augment=dict(rotate=, flip_dx=, flip_dy=, flip_dz=) into results['semkitti_voxels']; results['gt_occ'] = None.  The
+    training step then builds gt_occ on the GPU (targets.semantic_kitti_occupancy(..., augment=), through
+    OccupancyFormer.occupancy_targets); 'semkitti_voxels' must be collected into the img_metas.  Files of the wrong size
+    raise ValueError here.  Training pipelines only: is_train=False is refused (test pipelines take
+    LoadSemKittiVoxelFiles before LoadSemKittiAnnotation)."""
+
+    def __init__(self, bda_aug_conf, is_train=True, point_cloud_range=(0, -25.6, -2, 51.2, 25.6, 4.4),
+                 data_root="data/SemanticKITTI", data_info_path="projects/configs/_base_/semantickitti.yaml"):
+        if not is_train:
+            raise ValueError("LoadSemKittiVoxelFilesAug: is_train=False: this is the training-mode transform; test "
+                             "pipelines take LoadSemKittiVoxelFiles before LoadSemKittiAnnotation")
+        self.bda_aug_conf, self.is_train = bda_aug_conf, is_train
+        self.point_cloud_range = list(point_cloud_range)
+        self.learning_map = _learning_map(data_info_path)
+        self.data_root, self.data_info_path = data_root, data_info_path
+
+    def sample_bda_augmentation(self):
+        """the reference's five draws in its order -> (rotate, scale, flip_dx, flip_dy, flip_dz)"""
+        conf = self.bda_aug_conf
+        rotate = np.random.uniform(*conf["rot_lim"])
+        scale = np.random.uniform(*conf["scale_lim"])
+        flip_dx = np.random.uniform() < conf["flip_dx_ratio"]
+        flip_dy = np.random.uniform() < conf["flip_dy_ratio"]
+        flip_dz = np.random.uniform() < conf["flip_dz_ratio"]
+        return rotate, scale, flip_dx, flip_dy, flip_dz
+
+    def __call__(self, results):
+        vox = _voxel_files(self.data_root, results, self.learning_map)
+        rotate, _, flip_dx, flip_dy, flip_dz = self.sample_bda_augmentation()
+        bda_mat = semkitti_bda_matrix(rotate, flip_dx, flip_dy, flip_dz, self.point_cloud_range)
+        vox["augment"] = dict(rotate=float(rotate), flip_dx=bool(flip_dx), flip_dy=bool(flip_dy), flip_dz=bool(flip_dz))
+        results["semkitti_voxels"] = vox
+        results["gt_occ"] = None
+        imgs, rots, trans, intrins, post_rots, post_trans, gt_depths, sensor2sensors = results["img_inputs"]
+        results["img_inputs"] = (imgs, rots, trans, intrins, post_rots, post_trans, bda_mat, gt_depths, sensor2sensors)
         return results

@@ -16,7 +16,12 @@ SemanticKITTI's ground truth comes from the dataset's own voxel files instead of
                                + LoadSemKittiAnnotation's .long()     P/datasets/pipelines/loading_kitti_occ.py:34-53
 
 The 4 MB .label and 256 KB .invalid files of a frame cross PCIe instead of the 16 MB int64 volume, and the kernel
-(occ_semkitti_labels, csrc/semkitti_labels.cu) remaps and masks them in one pass.
+(occ_semkitti_labels, csrc/semkitti_labels.cu) remaps and masks them in one pass.  In training pipelines
+(semantic_kitti_occupancy(..., augment=)) one launch of another kernel also applies LoadSemKittiAnnotation's
+augmentation:
+
+    + voxel_transform's slice rotation and flips   P/datasets/pipelines/loading_kitti_occ.py:55-117,
+                                                    loading_nusc_occ.py:206-225 (occ_semkitti_labels_aug)
 """
 import numpy as np
 import torch
@@ -94,14 +99,34 @@ def _bytes(x, size, what, name):
     return m
 
 
-def semantic_kitti_occupancy(labels, invalids, learning_map, names=None):
+def semkitti_augment_rows(augment):
+    """per-sample augmentation dicts (rotate in degrees, flip_dx, flip_dy, flip_dz) -> int32 numpy (B, 10) rows of
+    occ_semkitti_labels_aug: the three flips, the rotate flag (not np.isclose(rotate, 0), as voxel_transform decides)
+    and the 16.16 coefficients of Image.rotate(rotate) of a 256 x 256 slice (image_prep.rotate_coeffs)"""
+    from .image_prep import rotate_coeffs
+    rows = []
+    for a in augment:
+        angle = float(a["rotate"])
+        rot = not np.isclose(angle, 0)
+        coeffs = rotate_coeffs(angle, SEMKITTI_SHAPE[1], SEMKITTI_SHAPE[0]) if rot else (1 << 16, 0, 0, 0, 1 << 16, 0)
+        rows.append([int(bool(a["flip_dx"])), int(bool(a["flip_dy"])), int(bool(a["flip_dz"])), int(rot), *coeffs])
+    return np.asarray(rows, dtype=np.int32).reshape(-1, 10)
+
+
+def semantic_kitti_occupancy(labels, invalids, learning_map, names=None, augment=None):
     """SemanticKITTI occupancy ground truth from the voxel files: labels / invalids = the bytes (bytes-like) of one
     sample's voxels/*.label and voxels/*.invalid, or lists of B of each; learning_map = the dataset yaml's -> int64 CUDA
     (256, 256, 32) (or (B, 256, 256, 32)) on the current device, equal to the reference's
     torch.tensor(np.load('<frame>_1_1.npy')).long(): remap_lut[label], then 255 where the invalid bit is set.  The files
     travel in one host-to-device copy from a pinned staging buffer kept per device.  A file of the wrong size, or a label
     at or past the LUT (the reference's IndexError; one count read back), raises ValueError naming the file (names: B
-    (.label name, .invalid name) pairs for the messages; default: the sample index)."""
+    (.label name, .invalid name) pairs for the messages; default: the sample index).
+
+    augment: None, or one dict per sample with 'rotate' (degrees), 'flip_dx', 'flip_dy', 'flip_dz', as
+    pipelines.LoadSemKittiVoxelFilesAug draws them -> the volume LoadSemKittiAnnotation(is_train=True) returns from the
+    same files: each z slice rotated as Pillow's Image.rotate(rotate, NEAREST, fillcolor=255) when not
+    np.isclose(rotate, 0), then the flips (occ_semkitti_labels_aug, one launch).  The learning map's values must then
+    lie in [0, 255], the reference's uint8 cast."""
     single = not isinstance(labels, (list, tuple))
     labels = [labels] if single else list(labels)
     invalids = [invalids] if single else list(invalids)
@@ -114,6 +139,14 @@ def semantic_kitti_occupancy(labels, invalids, learning_map, names=None):
     lab = [_bytes(x, SEMKITTI_LABEL_BYTES, ".label", n[0]) for x, n in zip(labels, names)]
     inv = [_bytes(x, SEMKITTI_INVALID_BYTES, ".invalid", n[1]) for x, n in zip(invalids, names)]
     lut = semkitti_remap_lut(learning_map)
+    if augment is not None:
+        augment = list(augment)
+        if len(augment) != B:
+            raise ValueError(f"semantic_kitti_occupancy: augment needs one dict per sample, got {len(augment)} for {B}")
+        if lut.min() < 0 or lut.max() > 255:
+            raise ValueError("semantic_kitti_occupancy: with augment, the learning map's values must lie in [0, 255] "
+                             "(voxel_transform casts the volume to uint8)")
+        aug = semkitti_augment_rows(augment)
     if not torch.cuda.is_available():
         raise RuntimeError("occformer_b200.targets: semantic_kitti_occupancy needs a CUDA device (no CPU fallback exists)")
     dev = torch.device("cuda", torch.cuda.current_device())
@@ -124,6 +157,9 @@ def semantic_kitti_occupancy(labels, invalids, learning_map, names=None):
         _semkitti_luts[key] = lut_d
     split = B * SEMKITTI_LABEL_BYTES
     total = split + B * SEMKITTI_INVALID_BYTES
+    aug_at = total
+    if augment is not None:
+        total += aug.nbytes  # the augmentation rows travel in the same copy, after the files
     staging, copied = _semkitti_staging.get(str(dev), (None, None))
     if staging is None or staging.numel() < total:
         staging, copied = torch.empty(total, dtype=torch.uint8, pin_memory=True), torch.cuda.Event()
@@ -134,11 +170,16 @@ def semantic_kitti_occupancy(labels, invalids, learning_map, names=None):
         hv[b * SEMKITTI_LABEL_BYTES:(b + 1) * SEMKITTI_LABEL_BYTES] = np.frombuffer(lab[b], np.uint8)
         o = split + b * SEMKITTI_INVALID_BYTES
         hv[o:o + SEMKITTI_INVALID_BYTES] = np.frombuffer(inv[b], np.uint8)
+    if augment is not None:
+        hv[aug_at:total] = aug.reshape(-1).view(np.uint8)
     data = host.to(dev, non_blocking=True)
     copied.record()
     _semkitti_staging[str(dev)] = (staging, copied)
     nvox = SEMKITTI_LABEL_BYTES // 2
-    vol, bad = ops.semkitti_labels(data[:split], data[split:], B, nvox, lut_d)
+    if augment is None:
+        vol, bad = ops.semkitti_labels(data[:split], data[split:], B, nvox, lut_d)
+    else:
+        vol, bad = ops.semkitti_labels_aug(data[:split], data[split:aug_at], B, data[aug_at:].view(torch.int32), lut_d)
     bad = bad.cpu()  # the one host synchronisation
     if bool(bad.any()):
         b = int(bad.nonzero()[0, 0])
