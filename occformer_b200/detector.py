@@ -124,15 +124,11 @@ class OccupancyFormer(nn.Module):
         'img_aug' of each sample's metas.  An empty uint8 (B, N, 0) imgs is LoadMultiViewJpegBytes_OccFormer's
         placeholder: the JPEG files in each 'img_aug' are decoded on the GPU first (image_prep.decode_jpeg); so is
         LoadMultiViewPngBytes_SemanticKitti's (B, 1, 0) one, whose 'img_aug' carries PNG files (image_prep.decode_png)."""
-        imgs = img[0]
-        if image_prep.is_file_placeholder(imgs):
-            augs = [m.get("img_aug", {}) for m in img_metas] if img_metas is not None else []
-            imgs = image_prep.decode_files(augs)
-            if imgs is None:
-                raise ValueError("OccupancyFormer: the empty image placeholder needs each sample's 'img_aug' meta with "
-                                 "its 'jpeg' files, which LoadMultiViewJpegBytes_OccFormer produces, or its 'png' files, "
-                                 "which LoadMultiViewPngBytes_SemanticKitti produces; add 'img_aug' to Collect3D's "
-                                 "meta_keys")
+        imgs = image_prep.input_frames(
+            img[0], img_metas,
+            "OccupancyFormer: the empty image placeholder needs each sample's 'img_aug' meta with its 'jpeg' files, "
+            "which LoadMultiViewJpegBytes_OccFormer produces, or its 'png' files, which "
+            "LoadMultiViewPngBytes_SemanticKitti produces; add 'img_aug' to Collect3D's meta_keys")
         if (imgs.dtype if torch.is_tensor(imgs) else imgs[0].dtype) == torch.uint8:
             if img_metas is None or any("img_aug" not in m for m in img_metas):
                 raise ValueError("OccupancyFormer: uint8 camera frames need each sample's 'img_aug' meta, which the "

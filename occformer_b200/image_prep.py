@@ -185,7 +185,7 @@ def lidar_depth_maps(points, img_inputs, img_aug):
     if all(p.is_cuda for p in pts):
         flat = torch.cat(pts).contiguous()
     else:
-        flat, _ = _stage([p.cpu().contiguous().numpy().view(np.uint8).reshape(-1) for p in pts])
+        flat, _ = ops._stage([p.cpu().contiguous().numpy().view(np.uint8).reshape(-1) for p in pts])
         flat = flat.view(torch.float32).view(-1, 3)
     inv_rots = torch.stack([torch.as_tensor(a["lidar_inv_rots"], dtype=torch.float32) for a in img_aug]).to(dev)
     return ops.lidar_depth(flat, offsets, inv_rots.contiguous(), trans.float().contiguous(),
@@ -210,74 +210,67 @@ def decode_files(img_aug):
     return decode([a[kind] for a in img_aug], None if None in names else names)
 
 
+def input_frames(imgs, img_metas, missing):
+    """img_inputs[0] -> the camera frames: the byte transforms' placeholder (is_file_placeholder) decoded from the files
+    in the 'img_aug' of img_metas (decode_files), anything else as it is; missing: the message of the ValueError raised
+    when the placeholder comes without files"""
+    if not is_file_placeholder(imgs):
+        return imgs
+    frames = decode_files([m.get("img_aug", {}) for m in img_metas or []])
+    if frames is None:
+        raise ValueError(missing)
+    return frames
+
+
 def camera_inputs(img_inputs, img_metas):
     """The reference training pipeline's collated img_inputs on the GPU, from those of LoadMultiViewImageFramesAug_* (or
     LoadMultiViewJpegBytesAug_OccFormer / LoadMultiViewPngBytesAug_SemanticKitti) + LoadLidarDepthPoints: img_inputs[0]
     the uint8 frames (prepare_images), or the byte transforms' empty placeholder, whose files are decoded first
-    (decode_files); the gt_depths placeholder (the slot before sensor2sensors: 6 of the loaders' 8-tuple, 7 once an
+    (input_frames); the gt_depths placeholder (the slot before sensor2sensors: 6 of the loaders' 8-tuple, 7 once an
     occupancy annotation transform has added bda_rot) replaced by lidar_depth_maps; every other element passed through.
     img_metas: B dicts carrying 'img_aug'."""
     img_aug = [m["img_aug"] for m in img_metas]
-    frames = img_inputs[0]
-    if is_file_placeholder(frames):
-        frames = decode_files(img_aug)
-        if frames is None:
-            raise ValueError("camera_inputs: the empty image placeholder needs each sample's 'img_aug' meta with its "
-                             "'jpeg' or 'png' files, which the byte transforms produce")
+    frames = input_frames(img_inputs[0], img_metas, "camera_inputs: the empty image placeholder needs each sample's "
+                          "'img_aug' meta with its 'jpeg' or 'png' files, which the byte transforms produce")
     imgs = prepare_images(frames, img_aug)
     depths = lidar_depth_maps([a["lidar_points"] for a in img_aug], img_inputs, img_aug)
     k = len(img_inputs) - 2
     return (imgs,) + tuple(img_inputs[1:k]) + (depths,) + tuple(img_inputs[k + 1:])
 
 
-def decode_jpeg(files, names=None, seq_bits=ops.JPEG_SEQ_BITS, sync_rounds=ops.JPEG_SYNC_ROUNDS):
-    """files: B samples, each a list of N JPEG files (bytes-like) -> uint8 CUDA (B, N, H, W, 3) B, G, R frames when all
-    share one size, else a list of B per-sample (N, H_i, W_i, 3) tensors: the two forms prepare_images takes, equal to
-    cv2.imdecode(buf, IMREAD_UNCHANGED) of each file.  The files travel in one pinned host buffer and one host-to-device
-    copy, and decode in one occ_decode_jpeg call; one status read-back then raises ValueError naming a file whose
-    entropy-coded data is corrupt (libjpeg would warn and fill in grey).  names: the same nesting of file names for the
-    messages (default: sample and camera indices).  seq_bits / sync_rounds tune the parallel Huffman decode and do not
-    change the result."""
+def _decode(what, files, names, parse, error, payload, decode, complaint, status_bits):
+    """the front end of decode_jpeg / decode_png (what): files B samples of N files, each parsed on the host by parse
+    (its error, an exception class, re-raised as ValueError naming the file) into a header; payload(file as a uint8
+    memoryview, header) -> the file's bytes to stage; decode(headers, payloads) -> (flat frames, int32 (M, 2) status)
+    of ops.decode_*.  One status read-back then raises ValueError naming the first file whose status is not 0 with
+    complaint and the names of its status_bits ((bit, name) pairs) -> the frames as _frames gives them"""
     samples = [list(s) for s in files]
     if not samples or any(not s for s in samples):
-        raise ValueError("decode_jpeg: needs at least one sample of at least one file")
+        raise ValueError(f"{what}: needs at least one sample of at least one file")
     label = [[names[b][n] if names is not None else f"sample {b} camera {n}" for n in range(len(s))]
              for b, s in enumerate(samples)]
-    headers, flat = [], []
+    headers, payloads = [], []
     for s, lab in zip(samples, label):
         for f, name in zip(s, lab):
             try:
-                headers.append(jpeg.parse(f))
-            except jpeg.JpegError as e:
-                raise ValueError(f"decode_jpeg: {name}: {e}") from None
-            flat.append(memoryview(f).cast("B"))
-    for s, lab, b0 in zip(samples, label, np.cumsum([0] + [len(s) for s in samples])[:-1]):
-        sizes = {(h.height, h.width) for h in headers[b0:b0 + len(s)]}
+                h = parse(f)
+            except error as e:
+                raise ValueError(f"{what}: {name}: {e}") from None
+            headers.append(h)
+            payloads += payload(memoryview(f).cast("B"), h)
+    first = np.cumsum([0] + [len(s) for s in samples])  # each sample's first image, then M
+    for b0, b1 in zip(first[:-1], first[1:]):
+        sizes = {(h.height, h.width) for h in headers[b0:b1]}
         if len(sizes) != 1:
-            raise ValueError(f"decode_jpeg: the cameras of a sample need one frame size, got {sorted(sizes)}")
-    data, offsets = _stage(flat)
-    out, status = ops.decode_jpeg(data, offsets, headers, seq_bits, sync_rounds)
+            raise ValueError(f"{what}: the cameras of a sample need one frame size, got {sorted(sizes)}")
+    out, status = decode(headers, payloads)
     bad = status[:, 0].cpu()
     if bool(bad.any()):
         m = int(bad.nonzero()[0, 0])
-        b = int(np.searchsorted(np.cumsum([len(s) for s in samples]), m, side="right"))
-        n = m - sum(len(s) for s in samples[:b])
-        raise ValueError(f"decode_jpeg: {label[b][n]}: corrupt entropy-coded data (status {int(bad[m])}: "
-                         + ", ".join(w for bit, w in ((1, "unexpected marker"), (2, "bad restart markers"),
-                                                      (4, "invalid Huffman code or run"), (8, "data ends early"))
-                                     if int(bad[m]) & bit) + ")")
+        b = int(np.searchsorted(first[1:], m, side="right"))
+        raise ValueError(f"{what}: {label[b][m - first[b]]}: {complaint} (status {int(bad[m])}: "
+                         + ", ".join(w for bit, w in status_bits if int(bad[m]) & bit) + ")")
     return _frames(out, samples, headers)
-
-
-def _stage(pieces):
-    """bytes-like pieces -> (uint8 CUDA buffer holding them back to back, each piece's byte offset): one pinned host
-    buffer and one host-to-device copy"""
-    offsets = np.cumsum([0] + [len(f) for f in pieces]).tolist()
-    host = torch.empty(offsets[-1], dtype=torch.uint8, pin_memory=True)
-    hv = host.numpy()
-    for f, o in zip(pieces, offsets):
-        hv[o:o + len(f)] = np.frombuffer(f, np.uint8)
-    return host.to(torch.cuda.current_device(), non_blocking=True), offsets[:-1]
 
 
 def _frames(out, samples, headers):
@@ -294,6 +287,25 @@ def _frames(out, samples, headers):
     return res
 
 
+JPEG_STATUS = ((1, "unexpected marker"), (2, "bad restart markers"), (4, "invalid Huffman code or run"),
+               (8, "data ends early"))
+
+
+def decode_jpeg(files, names=None, seq_bits=ops.JPEG_SEQ_BITS, sync_rounds=ops.JPEG_SYNC_ROUNDS):
+    """files: B samples, each a list of N JPEG files (bytes-like) -> uint8 CUDA (B, N, H, W, 3) B, G, R frames when all
+    share one size, else a list of B per-sample (N, H_i, W_i, 3) tensors: the two forms prepare_images takes, equal to
+    cv2.imdecode(buf, IMREAD_UNCHANGED) of each file.  The files travel in one pinned host buffer and one host-to-device
+    copy, and decode in one occ_decode_jpeg call; one status read-back then raises ValueError naming a file whose
+    entropy-coded data is corrupt (libjpeg would warn and fill in grey).  names: the same nesting of file names for the
+    messages (default: sample and camera indices).  seq_bits / sync_rounds tune the parallel Huffman decode and do not
+    change the result."""
+    def decode(headers, payloads):
+        data, offsets = ops._stage(payloads)
+        return ops.decode_jpeg(data, offsets, headers, seq_bits, sync_rounds)
+    return _decode("decode_jpeg", files, names, jpeg.parse, jpeg.JpegError, lambda f, h: [f], decode,
+                   "corrupt entropy-coded data", JPEG_STATUS)
+
+
 PNG_STATUS = ((1, "invalid deflate data"), (2, "data ends early or too little image data"),
               (4, "incorrect Adler-32 check"), (8, "bad filter type"))
 
@@ -306,38 +318,13 @@ def decode_png(files, names=None):
     one host-to-device copy, and decode in one occ_decode_png call; one status read-back then raises ValueError naming
     a file cv2 would not decode.  names: the same nesting of file names for the messages (default: sample and camera
     indices)."""
-    samples = [list(s) for s in files]
-    if not samples or any(not s for s in samples):
-        raise ValueError("decode_png: needs at least one sample of at least one file")
-    label = [[names[b][n] if names is not None else f"sample {b} camera {n}" for n in range(len(s))]
-             for b, s in enumerate(samples)]
-    headers, pieces, starts = [], [], []
-    for s, lab in zip(samples, label):
-        for f, name in zip(s, lab):
-            try:
-                h = png.parse(f)
-            except png.PngError as e:
-                raise ValueError(f"decode_png: {name}: {e}") from None
-            headers.append(h)
-            v = memoryview(f).cast("B")
-            pieces += [v[o:o + n] for o, n in h.idat]
-            starts += np.cumsum([0] + [n for _, n in h.idat])[:-1].tolist()
-    for s, lab, b0 in zip(samples, label, np.cumsum([0] + [len(s) for s in samples])[:-1]):
-        sizes = {(h.height, h.width) for h in headers[b0:b0 + len(s)]}
-        if len(sizes) != 1:
-            raise ValueError(f"decode_png: the cameras of a sample need one frame size, got {sorted(sizes)}")
-    streams = sum((h.stream_len for h in headers), 0)
-    pad = -streams % 4
-    pieces += [bytes(pad), np.asarray(starts, np.int32).tobytes()]
-    data, offsets = _stage(pieces)
-    stream_off = np.cumsum([0] + [h.stream_len for h in headers])[:-1].tolist()
-    idat = data[streams + pad:].view(torch.int32)
-    out, status = ops.decode_png(data[:max(streams, 1)], stream_off, headers, idat)
-    bad = status[:, 0].cpu()
-    if bool(bad.any()):
-        m = int(bad.nonzero()[0, 0])
-        b = int(np.searchsorted(np.cumsum([len(s) for s in samples]), m, side="right"))
-        n = m - sum(len(s) for s in samples[:b])
-        raise ValueError(f"decode_png: {label[b][n]}: cv2 would not decode it (status {int(bad[m])}: "
-                         + ", ".join(w for bit, w in PNG_STATUS if int(bad[m]) & bit) + ")")
-    return _frames(out, samples, headers)
+    def decode(headers, payloads):
+        starts = [s for h in headers for s in np.cumsum([0] + [n for _, n in h.idat])[:-1].tolist()]
+        streams = sum((h.stream_len for h in headers), 0)
+        pad = -streams % 4
+        data, _ = ops._stage(payloads + [bytes(pad), np.asarray(starts, np.int32).tobytes()])
+        stream_off = np.cumsum([0] + [h.stream_len for h in headers])[:-1].tolist()
+        idat = data[streams + pad:].view(torch.int32)
+        return ops.decode_png(data[:max(streams, 1)], stream_off, headers, idat)
+    return _decode("decode_png", files, names, png.parse, png.PngError, lambda f, h: [f[o:o + n] for o, n in h.idat],
+                   decode, "cv2 would not decode it", PNG_STATUS)

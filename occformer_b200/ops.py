@@ -6,6 +6,7 @@ non-zero return code.  No fallback paths.
 """
 import ctypes
 
+import numpy as np
 import torch
 
 from ._lib import check, lib, parameters
@@ -27,6 +28,45 @@ LAUNCH_COUNT = _LaunchCount()
 def _stream():
     """the current torch stream of the current device (where _checked requires a call's tensors to live)"""
     return torch.cuda.current_stream().cuda_stream
+
+
+# ----------------------------------------------------------------------------------------------- host-side caches
+_stream_ws = {}      # (kernel, device, stream) -> (grow-only uint8 workspace, superseded workspaces)
+_device_tables = {}  # (device, key) -> constant table on the device
+
+
+def _stream_workspace(kernel, dev, nbytes):
+    """kernel's grow-only uint8 workspace for the current stream of dev, at least nbytes long"""
+    key = (kernel, str(dev), torch.cuda.current_stream(dev).cuda_stream)
+    ent = _stream_ws.get(key)
+    if ent is None or ent[0].numel() < nbytes:
+        # a graph captured before the workspace grew still points at the old one: keep it referenced
+        old = [] if ent is None else ent[1] + [ent[0]]
+        ent = (torch.empty(nbytes, dtype=torch.uint8, device=dev), old)
+        _stream_ws[key] = ent
+    return ent[0]
+
+
+def _device_table(dev, key, make):
+    """the device copy of the numpy array make() returns, built on first use per (dev, key); key stands for the content"""
+    k = (str(dev), key)
+    t = _device_tables.get(k)
+    if t is None:
+        t = torch.from_numpy(make()).to(dev)
+        _device_tables[k] = t
+    return t
+
+
+def _stage(pieces):
+    """bytes-like pieces -> (uint8 CUDA buffer of the current device holding them back to back, each piece's byte
+    offset): one pinned host buffer, which torch's caching host allocator recycles once the copy is done, and one
+    host-to-device copy"""
+    offsets = np.cumsum([0] + [len(f) for f in pieces]).tolist()
+    host = torch.empty(offsets[-1], dtype=torch.uint8, pin_memory=True)
+    hv = host.numpy()
+    for f, o in zip(pieces, offsets):
+        hv[o:o + len(f)] = np.frombuffer(f, np.uint8)
+    return host.to(torch.cuda.current_device(), non_blocking=True), offsets[:-1]
 
 
 # tensor dtype per pointee type of the header (S32 is a float32 container; void: any; size_t* is host-only: no tensor)
@@ -900,21 +940,6 @@ def ssc_counts(pred, target, K, ignore=255):
     return out
 
 
-_pan_ws = {}  # (device, stream) -> grow-only uint8 workspace of occ_panoptic_eval
-
-
-def _panoptic_eval_ws(n, device):
-    key = (str(device), torch.cuda.current_stream(device).cuda_stream)
-    nbytes = lib().occ_panoptic_eval_workspace_bytes(n)
-    if nbytes == 0:
-        raise RuntimeError(f"occformer_b200: panoptic evaluation of {n} elements exceeds the 2^29-element limit of one call")
-    ws = _pan_ws.get(key)
-    if ws is None or ws.numel() < nbytes:
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=device)  # zeroed by every call
-        _pan_ws[key] = ws
-    return ws
-
-
 def _flat_ids(t, name):
     """integer (or whole-number floating) tensor of any shape -> flat contiguous int64"""
     if t.dtype == torch.bool or t.is_complex():
@@ -933,7 +958,10 @@ def panoptic_eval(x_sem, x_inst, y_sem, y_inst, K, ignore_mask, min_points, stat
     if any(t is not None and t.numel() != n for t in (ys, xi, yi)):
         raise RuntimeError("occformer_b200: panoptic_eval inputs must have the same number of elements")
     assert state.numel() == K * K + 6 * K + 1, "panoptic state vector has the wrong length"
-    ws = _panoptic_eval_ws(n, xs.device)
+    nbytes = lib().occ_panoptic_eval_workspace_bytes(n)
+    if nbytes == 0:
+        raise RuntimeError(f"occformer_b200: panoptic evaluation of {n} elements exceeds the 2^29-element limit of one call")
+    ws = _stream_workspace("occ_panoptic_eval", xs.device, nbytes)  # zeroed by every call
     _call("occ_panoptic_eval", xs, xi, ys, yi, n, K, ignore_mask, min_points, parts, ws, ws.numel(), state)
     return state
 
@@ -947,9 +975,6 @@ def lidarseg_hist(scores, labels, K, hist=None):
 
 
 # ----------------------------------------------------------------------------------------------- occupancy ground truth
-_targets_ws = {}  # (device, stream) -> grow-only uint8 workspace of occ_lidarseg_occupancy
-
-
 def lidarseg_occupancy(pts, counts, pc_range, grid, panoptic, empty_id, ignore):
     """Occupancy ground truth of B samples (occ_lidarseg_occupancy): pts (n, ld >= 4) fp32 CUDA rows [x, y, z, label, ...],
     sample b the next counts[b] rows -> (int64 (B, X, Y, Z) volume, int32 (1,) invalid-point counter); no synchronisation."""
@@ -965,11 +990,7 @@ def lidarseg_occupancy(pts, counts, pc_range, grid, panoptic, empty_id, ignore):
     if nbytes == 0:
         raise RuntimeError(f"occformer_b200: occ_lidarseg_occupancy takes 1..256 samples and at most 2^30 points, "
                            f"got {B} samples, {n} points")
-    key = (str(dev), torch.cuda.current_stream(dev).cuda_stream)
-    ws = _targets_ws.get(key)
-    if ws is None or ws.numel() < nbytes:
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        _targets_ws[key] = ws
+    ws = _stream_workspace("occ_lidarseg_occupancy", dev, nbytes)
     out = torch.empty((B, X, Y, Z), dtype=torch.int64, device=dev)
     invalid = torch.zeros(1, dtype=torch.int32, device=dev)
     r = [float(v) for v in pc_range]
@@ -1004,19 +1025,15 @@ def semkitti_labels_aug(label, invalid, B, aug, lut):
 
 
 # ----------------------------------------------------------------------------------------------- camera images
-_prep_tables = {}  # (device, source size, resized size) -> int32 resample table of one axis (image_prep.resample_table)
-_prep_norms = {}   # (device, mean, std, to_rgb) -> float32 (3, 256) normalisation table
-_prep_ws = {}      # (device, stream) -> grow-only uint8 workspace of occ_prepare_images
+def _image_prep():
+    from . import image_prep  # image_prep imports ops at its top, so ops imports image_prep at call time
+    return image_prep
 
 
 def _prep_table(dev, in_size, out_size):
-    key = (str(dev), in_size, out_size)
-    t = _prep_tables.get(key)
-    if t is None:
-        from .image_prep import resample_table
-        t = torch.from_numpy(resample_table(in_size, out_size)).to(dev)
-        _prep_tables[key] = t
-    return t
+    """the int32 resample table of one axis (image_prep.resample_table) on dev"""
+    return _device_table(dev, ("resample", in_size, out_size),
+                         lambda: _image_prep().resample_table(in_size, out_size))
 
 
 def prepare_images(frames, offsets, geoms, input_size, mean, std, to_rgb, aug=None):
@@ -1028,21 +1045,13 @@ def prepare_images(frames, offsets, geoms, input_size, mean, std, to_rgb, aug=No
     fH, fW = (int(v) for v in input_size)
     dev = frames.device
     geom = (ctypes.c_int * (6 * M))(*[int(v) for g in geoms for v in g])
-    nkey = (str(dev), tuple(mean), tuple(std), bool(to_rgb))
-    norm = _prep_norms.get(nkey)
-    if norm is None:
-        from .image_prep import normalize_table
-        norm = torch.from_numpy(normalize_table(mean, std, to_rgb)).to(dev)
-        _prep_norms[nkey] = norm
+    norm = _device_table(dev, ("normalize", tuple(mean), tuple(std), bool(to_rgb)),
+                         lambda: _image_prep().normalize_table(mean, std, to_rgb))
     tables = []
     for H, W, rW, rH, _, _ in geoms:
         tables += [_prep_table(dev, W, rW).data_ptr(), _prep_table(dev, H, rH).data_ptr()]
     nbytes = lib().occ_prepare_images_workspace_bytes(geom, M, fH, fW)
-    key = (str(dev), torch.cuda.current_stream(dev).cuda_stream)
-    ws = _prep_ws.get(key)
-    if ws is None or ws.numel() < max(nbytes, 16):
-        ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
-        _prep_ws[key] = ws
+    ws = _stream_workspace("occ_prepare_images", dev, max(nbytes, 16))
     out = torch.empty((M, 3, fH, fW), dtype=torch.float32, device=dev)
     head = [frames, frames.numel(), (ctypes.c_longlong * M)(*offsets), geom]
     tail = [M, fH, fW, (ctypes.c_longlong * (2 * M))(*tables), norm, int(bool(to_rgb)), ws, ws.numel(), out]
@@ -1069,29 +1078,11 @@ def lidar_depth(pts, offsets, inv_rots, trans, intrins, post_rots, post_trans, i
 JPEG_SEQ_BITS = 4096    # bits per subsequence of the parallel Huffman decode (scripts/bench_jpeg.py --tune)
 JPEG_SYNC_ROUNDS = 6    # self-synchronisation rounds before the serial fix-up
 JPEG_MAX_IMAGES = 96    # images per occ_decode_jpeg call
-_jpeg_tables = {}       # (device, DQT / DHT bytes) -> int32 table on the device
-_jpeg_ws = {}           # (device, stream) -> (grow-only uint8 workspace of occ_decode_jpeg, superseded workspaces)
 
 
 def _jpeg_table(dev, key, table):
-    k = (str(dev), key)
-    t = _jpeg_tables.get(k)
-    if t is None:
-        t = torch.from_numpy(table).to(dev)
-        _jpeg_tables[k] = t
-    return t
-
-
-def _stream_workspace(cache, dev, nbytes):
-    """the grow-only uint8 workspace of cache for the current stream of dev, at least nbytes long"""
-    key = (str(dev), torch.cuda.current_stream(dev).cuda_stream)
-    ent = cache.get(key)
-    if ent is None or ent[0].numel() < nbytes:
-        # a graph captured before the workspace grew still points at the old one: keep it referenced
-        old = [] if ent is None else ent[1] + [ent[0]]
-        ent = (torch.empty(nbytes, dtype=torch.uint8, device=dev), old)
-        cache[key] = ent
-    return ent[0]
+    """a DQT / DHT table of jpeg.parse (key: its marker bytes, table: int32 numpy) on dev"""
+    return _device_table(dev, key, lambda: table)
 
 
 def decode_jpeg(data, offsets, headers, seq_bits=JPEG_SEQ_BITS, sync_rounds=JPEG_SYNC_ROUNDS):
@@ -1107,9 +1098,7 @@ def decode_jpeg(data, offsets, headers, seq_bits=JPEG_SEQ_BITS, sync_rounds=JPEG
     for off, h in zip(offsets, headers):
         scan += [int(off) + h.scan_off, h.scan_len]
         geom += [h.height, h.width, h.hs, h.vs, h.restart]
-        tables += [_jpeg_table(dev, *q).data_ptr() for q in h.qt]
-        tables += [_jpeg_table(dev, *t).data_ptr() for t in h.dc]
-        tables += [_jpeg_table(dev, *t).data_ptr() for t in h.ac]
+        tables += [_jpeg_table(dev, *t).data_ptr() for t in h.qt + h.dc + h.ac]
         out_off.append(total)
         total += h.height * h.width * 3
     scan = (ctypes.c_longlong * (2 * M))(*scan)
@@ -1117,7 +1106,7 @@ def decode_jpeg(data, offsets, headers, seq_bits=JPEG_SEQ_BITS, sync_rounds=JPEG
     nbytes = lib().occ_decode_jpeg_workspace_bytes(scan, geom, M, int(seq_bits))
     if nbytes == 0:
         raise RuntimeError(f"occformer_b200: occ_decode_jpeg takes 32 <= seq_bits <= 2^20, got {seq_bits}")
-    ws = _stream_workspace(_jpeg_ws, dev, nbytes)
+    ws = _stream_workspace("occ_decode_jpeg", dev, nbytes)
     out = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)
     status = torch.empty((M, 2), dtype=torch.int32, device=dev)
     _call("occ_decode_jpeg", data, data.numel(), scan, geom, (ctypes.c_longlong * (9 * M))(*tables),
@@ -1129,7 +1118,6 @@ def decode_jpeg(data, offsets, headers, seq_bits=JPEG_SEQ_BITS, sync_rounds=JPEG
 # ----------------------------------------------------------------------------------------------- PNG decoding
 PNG_MAX_IMAGES = 96     # images per occ_decode_png call
 PNG_LAUNCHES = 37       # enqueued launches and memsets per call (include/occ_b200.h)
-_png_ws = {}            # (device, stream) -> (grow-only uint8 workspace of occ_decode_png, superseded workspaces)
 
 
 def decode_png(data, offsets, headers, idat):
@@ -1152,7 +1140,7 @@ def decode_png(data, offsets, headers, idat):
     nbytes = lib().occ_decode_png_workspace_bytes(streams, geom, counts, M)
     if nbytes == 0:
         raise RuntimeError("occformer_b200: occ_decode_png refused the geometry or the streams")
-    ws = _stream_workspace(_png_ws, dev, nbytes)
+    ws = _stream_workspace("occ_decode_png", dev, nbytes)
     out = torch.empty(max(total, 1), dtype=torch.uint8, device=dev)
     status = torch.empty((M, 2), dtype=torch.int32, device=dev)
     _call("occ_decode_png", data, data.numel(), streams, geom, counts, idat, idat.numel(),

@@ -20,6 +20,7 @@ import os
 import numpy as np
 import torch
 
+from . import jpeg, png
 from .registry import PIPELINES
 
 
@@ -203,9 +204,18 @@ class _ImageFrames:
             raise ValueError(f"{path}: a 3-channel uint8 frame is needed, got {img.dtype} {img.shape}")
         return img
 
-    def camera(self, img):
-        """one decoded frame -> (resize_dims, crop, flip, rotate, post_rot, post_tran)"""
-        return self.camera_size(img.shape[0], img.shape[1])
+    def load(self, path):
+        """one camera's file -> (its payload, (H, W)): the decoded frame"""
+        img = self.decode(path)
+        return img, img.shape[:2]
+
+    def image_input(self, payloads):
+        """img_inputs[0] of a sample from its cameras' payloads: the uint8 (N, H, W, 3) frames"""
+        return torch.stack([torch.from_numpy(p) for p in payloads])
+
+    def file_meta(self, payloads, paths):
+        """what results['img_aug'] carries besides the augmentation: nothing"""
+        return {}
 
     def camera_size(self, H, W):
         """one camera of an H x W frame -> (resize_dims, crop, flip, rotate, post_rot, post_tran)"""
@@ -234,15 +244,17 @@ class LoadMultiViewImageFrames_OccFormer(_ImageFrames):
     def __call__(self, results):
         cam_names = self.choose_cams()
         results["cam_names"] = cam_names
-        frames, rots, trans, intrins, post_rots, post_trans, sensor2sensors, dims, crops, flips, rotates = (
-            [] for _ in range(11))
+        payloads, paths, sizes, rots, trans, intrins, post_rots, post_trans, sensor2sensors, dims, crops, flips, \
+            rotates = ([] for _ in range(13))
         for cam_name in cam_names:
             cam_data = results["curr"]["cams"][cam_name]
-            img = self.decode(cam_data["data_path"])
+            payload, (H, W) = self.load(cam_data["data_path"])
             intrin = torch.Tensor(cam_data["cam_intrinsic"])
             sensor2lidar = torch.tensor(results["lidar2cam_dic"][cam_name]).inverse().float()
-            resize_dims, crop, flip, rotate, post_rot, post_tran = self.camera(img)
-            frames.append(torch.from_numpy(img))
+            resize_dims, crop, flip, rotate, post_rot, post_tran = self.camera_size(H, W)
+            payloads.append(payload)
+            paths.append(cam_data["data_path"])
+            sizes.append((H, W))
             intrins.append(intrin)
             rots.append(sensor2lidar[:3, :3])
             trans.append(sensor2lidar[:3, 3])
@@ -253,12 +265,12 @@ class LoadMultiViewImageFrames_OccFormer(_ImageFrames):
             crops.append(crop)
             flips.append(flip)
             rotates.append(rotate)
-        if len({tuple(f.shape) for f in frames}) != 1:
+        if len(set(sizes)) != 1:
             raise ValueError(f"{type(self).__name__}: the cameras of a sample need one frame size")
         gt_depths = [torch.zeros(1) for _ in cam_names]
-        results["img_inputs"] = tuple(torch.stack(x) for x in (frames, rots, trans, intrins, post_rots, post_trans,
-                                                                gt_depths, sensor2sensors))
-        results["img_aug"] = self.img_aug(dims, crops, flips, rotates)
+        results["img_inputs"] = (self.image_input(payloads),) + tuple(
+            torch.stack(x) for x in (rots, trans, intrins, post_rots, post_trans, gt_depths, sensor2sensors))
+        results["img_aug"] = dict(self.img_aug(dims, crops, flips, rotates), **self.file_meta(payloads, paths))
         return results
 
 
@@ -268,19 +280,22 @@ class LoadMultiViewImageFrames_SemanticKitti(_ImageFrames):
     and normalisation to the GPU: img_inputs[0] is the decoded uint8 (1, H, W, 3) BGR frame, img_inputs[1:] are the
     reference's, results['raw_img'] is kept and results['img_aug'] added; results['canvas'] is not produced."""
 
+    keep_raw_img = True  # results['raw_img'] = the decoded frame
+
     def __call__(self, results):
         img_filenames = results["img_filename"]
         assert len(img_filenames) == 1
-        img = self.decode(img_filenames[0])
-        results["raw_img"] = img
-        resize_dims, crop, flip, rotate, post_rot, post_tran = self.camera(img)
+        payload, (H, W) = self.load(img_filenames[0])
+        if self.keep_raw_img:
+            results["raw_img"] = payload
+        resize_dims, crop, flip, rotate, post_rot, post_tran = self.camera_size(H, W)
         intrin = torch.Tensor(results["cam_intrinsic"][0])
         lidar2cam = torch.Tensor(results["lidar2cam"][0])
         cam2lidar = lidar2cam.inverse()
-        res = [torch.from_numpy(img), cam2lidar[:3, :3], cam2lidar[:3, 3], intrin, post_rot, post_tran, torch.zeros(1),
-               cam2lidar]
-        results["img_inputs"] = tuple(x[None] for x in res)
-        results["img_aug"] = self.img_aug([resize_dims], [crop], [flip], [rotate])
+        res = [cam2lidar[:3, :3], cam2lidar[:3, 3], intrin, post_rot, post_tran, torch.zeros(1), cam2lidar]
+        results["img_inputs"] = (self.image_input([payload]),) + tuple(x[None] for x in res)
+        results["img_aug"] = dict(self.img_aug([resize_dims], [crop], [flip], [rotate]),
+                                  **self.file_meta([payload], [img_filenames[0]]))
         return results
 
 
@@ -335,8 +350,29 @@ class LoadLidarDepthPoints:
         return results
 
 
+class _FileBytes:
+    """the byte transforms' part (mixed into a frame transform): a camera's payload is its file's bytes and (H, W) comes
+    from the file's header (frame_size, whose error names the file in a ValueError); img_inputs[0] is an empty
+    uint8 (N, 0) placeholder and results['img_aug'] also carries the files (kind) and their paths (kind + '_files').
+    The class sets kind, frame_size and error."""
+
+    def load(self, path):
+        with open(path, "rb") as f:
+            data = f.read()
+        try:
+            return data, self.frame_size(data)
+        except self.error as e:
+            raise ValueError(f"{path}: {e}") from None
+
+    def image_input(self, payloads):
+        return torch.zeros((len(payloads), 0), dtype=torch.uint8)
+
+    def file_meta(self, payloads, paths):
+        return {self.kind: list(payloads), self.kind + "_files": list(paths)}
+
+
 @PIPELINES.register_module()
-class LoadMultiViewJpegBytes_OccFormer(LoadMultiViewImageFrames_OccFormer):
+class LoadMultiViewJpegBytes_OccFormer(_FileBytes, LoadMultiViewImageFrames_OccFormer):
     """LoadMultiViewImageFrames_OccFormer without the decode: each camera file's bytes are read and the frame size comes
     from its SOF header (jpeg.frame_size), so img_aug and img_inputs[1:] are the frame transform's.  results['img_aug']
     also carries 'jpeg' (the N files' bytes, in camera order) and 'jpeg_files' (their paths); img_inputs[0] is an empty
@@ -344,48 +380,11 @@ class LoadMultiViewJpegBytes_OccFormer(LoadMultiViewImageFrames_OccFormer):
     decodes the files on the GPU (image_prep.decode_jpeg) and prepares the images from the frames.  Files the device
     decoder does not take (progressive, grayscale, ...) raise ValueError here, in the loader."""
 
-    def __call__(self, results):
-        from .jpeg import JpegError, frame_size
-        cam_names = self.choose_cams()
-        results["cam_names"] = cam_names
-        files, paths, rots, trans, intrins, post_rots, post_trans, sensor2sensors, dims, crops, sizes, flips, rotates = (
-            [] for _ in range(13))
-        for cam_name in cam_names:
-            cam_data = results["curr"]["cams"][cam_name]
-            path = cam_data["data_path"]
-            with open(path, "rb") as f:
-                data = f.read()
-            try:
-                H, W = frame_size(data)
-            except JpegError as e:
-                raise ValueError(f"{path}: {e}") from None
-            intrin = torch.Tensor(cam_data["cam_intrinsic"])
-            sensor2lidar = torch.tensor(results["lidar2cam_dic"][cam_name]).inverse().float()
-            resize_dims, crop, flip, rotate, post_rot, post_tran = self.camera_size(H, W)
-            files.append(data)
-            paths.append(path)
-            sizes.append((H, W))
-            intrins.append(intrin)
-            rots.append(sensor2lidar[:3, :3])
-            trans.append(sensor2lidar[:3, 3])
-            post_rots.append(post_rot)
-            post_trans.append(post_tran)
-            sensor2sensors.append(sensor2lidar)
-            dims.append(resize_dims)
-            crops.append(crop)
-            flips.append(flip)
-            rotates.append(rotate)
-        if len(set(sizes)) != 1:
-            raise ValueError(f"{type(self).__name__}: the cameras of a sample need one frame size")
-        gt_depths = [torch.zeros(1) for _ in cam_names]
-        results["img_inputs"] = (torch.zeros((len(cam_names), 0), dtype=torch.uint8),) + tuple(
-            torch.stack(x) for x in (rots, trans, intrins, post_rots, post_trans, gt_depths, sensor2sensors))
-        results["img_aug"] = dict(self.img_aug(dims, crops, flips, rotates), jpeg=files, jpeg_files=paths)
-        return results
+    kind, frame_size, error = "jpeg", staticmethod(jpeg.frame_size), jpeg.JpegError
 
 
 @PIPELINES.register_module()
-class LoadMultiViewPngBytes_SemanticKitti(LoadMultiViewImageFrames_SemanticKitti):
+class LoadMultiViewPngBytes_SemanticKitti(_FileBytes, LoadMultiViewImageFrames_SemanticKitti):
     """LoadMultiViewImageFrames_SemanticKitti without the decode: the frame file's bytes are read and the frame size
     comes from its IHDR chunk (png.frame_size), so img_aug and img_inputs[1:] are the frame transform's.
     results['img_aug'] also carries 'png' (the file's bytes, in a list of one) and 'png_files' (its path); img_inputs[0]
@@ -396,25 +395,8 @@ class LoadMultiViewPngBytes_SemanticKitti(LoadMultiViewImageFrames_SemanticKitti
     test loop (pred_save) reads it, and that keeps the frame transform.  Test pipelines only: is_train=True is refused,
     as the frame transform refuses it."""
 
-    def __call__(self, results):
-        from .png import PngError, frame_size
-        img_filenames = results["img_filename"]
-        assert len(img_filenames) == 1
-        path = img_filenames[0]
-        with open(path, "rb") as f:
-            data = f.read()
-        try:
-            H, W = frame_size(data)
-        except PngError as e:
-            raise ValueError(f"{path}: {e}") from None
-        resize_dims, crop, flip, rotate, post_rot, post_tran = self.camera_size(H, W)
-        intrin = torch.Tensor(results["cam_intrinsic"][0])
-        lidar2cam = torch.Tensor(results["lidar2cam"][0])
-        cam2lidar = lidar2cam.inverse()
-        res = [cam2lidar[:3, :3], cam2lidar[:3, 3], intrin, post_rot, post_tran, torch.zeros(1), cam2lidar]
-        results["img_inputs"] = (torch.zeros((1, 0), dtype=torch.uint8),) + tuple(x[None] for x in res)
-        results["img_aug"] = dict(self.img_aug([resize_dims], [crop], [flip], [rotate]), png=[data], png_files=[path])
-        return results
+    kind, frame_size, error = "png", staticmethod(png.frame_size), png.PngError
+    keep_raw_img = False
 
 
 @PIPELINES.register_module()

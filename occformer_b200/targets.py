@@ -75,8 +75,6 @@ def panoptic_occupancy(points, occ_size, point_cloud_range, unoccupied_id=17):
 SEMKITTI_SHAPE = (256, 256, 32)
 SEMKITTI_LABEL_BYTES = 2 * 256 * 256 * 32   # .label: one uint16 per voxel
 SEMKITTI_INVALID_BYTES = 256 * 256 * 32 // 8  # .invalid: one bit per voxel
-_semkitti_luts = {}  # (device, LUT bytes) -> int32 CUDA remap table
-_semkitti_staging = {}  # device -> (grow-only pinned uint8 buffer, CUDA event after its last host-to-device copy)
 
 
 def semkitti_remap_lut(learning_map):
@@ -118,7 +116,7 @@ def semantic_kitti_occupancy(labels, invalids, learning_map, names=None, augment
     sample's voxels/*.label and voxels/*.invalid, or lists of B of each; learning_map = the dataset yaml's -> int64 CUDA
     (256, 256, 32) (or (B, 256, 256, 32)) on the current device, equal to the reference's
     torch.tensor(np.load('<frame>_1_1.npy')).long(): remap_lut[label], then 255 where the invalid bit is set.  The files
-    travel in one host-to-device copy from a pinned staging buffer kept per device.  A file of the wrong size, or a label
+    travel in one pinned host buffer and one host-to-device copy (ops._stage).  A file of the wrong size, or a label
     at or past the LUT (the reference's IndexError; one count read back), raises ValueError naming the file (names: B
     (.label name, .invalid name) pairs for the messages; default: the sample index).
 
@@ -150,31 +148,11 @@ def semantic_kitti_occupancy(labels, invalids, learning_map, names=None, augment
     if not torch.cuda.is_available():
         raise RuntimeError("occformer_b200.targets: semantic_kitti_occupancy needs a CUDA device (no CPU fallback exists)")
     dev = torch.device("cuda", torch.cuda.current_device())
-    key = (str(dev), lut.tobytes())
-    lut_d = _semkitti_luts.get(key)
-    if lut_d is None:
-        lut_d = torch.from_numpy(lut).to(dev)
-        _semkitti_luts[key] = lut_d
+    lut_d = ops._device_table(dev, ("semkitti_lut", lut.tobytes()), lambda: lut)
+    # one copy: the labels, then the invalid bits, then the augmentation rows
+    data, _ = ops._stage(lab + inv + ([] if augment is None else [aug.reshape(-1).view(np.uint8)]))
     split = B * SEMKITTI_LABEL_BYTES
-    total = split + B * SEMKITTI_INVALID_BYTES
-    aug_at = total
-    if augment is not None:
-        total += aug.nbytes  # the augmentation rows travel in the same copy, after the files
-    staging, copied = _semkitti_staging.get(str(dev), (None, None))
-    if staging is None or staging.numel() < total:
-        staging, copied = torch.empty(total, dtype=torch.uint8, pin_memory=True), torch.cuda.Event()
-    copied.synchronize()  # the buffer's previous copy has left it (a no-op after the read-back of a finished call)
-    host = staging[:total]
-    hv = host.numpy()
-    for b in range(B):
-        hv[b * SEMKITTI_LABEL_BYTES:(b + 1) * SEMKITTI_LABEL_BYTES] = np.frombuffer(lab[b], np.uint8)
-        o = split + b * SEMKITTI_INVALID_BYTES
-        hv[o:o + SEMKITTI_INVALID_BYTES] = np.frombuffer(inv[b], np.uint8)
-    if augment is not None:
-        hv[aug_at:total] = aug.reshape(-1).view(np.uint8)
-    data = host.to(dev, non_blocking=True)
-    copied.record()
-    _semkitti_staging[str(dev)] = (staging, copied)
+    aug_at = split + B * SEMKITTI_INVALID_BYTES
     nvox = SEMKITTI_LABEL_BYTES // 2
     if augment is None:
         vol, bad = ops.semkitti_labels(data[:split], data[split:], B, nvox, lut_d)

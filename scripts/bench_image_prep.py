@@ -137,7 +137,7 @@ def main():
         for _ in range(5):
             t = time.perf_counter()
             for f in frames:
-                tr.camera(f)
+                tr.camera_size(*f.shape[:2])
             torch.from_numpy(np.stack(frames))
             tn.append((time.perf_counter() - t) * 1e3)
         print(f"  {name} host per sample, one thread: reference steps 2-4 (Pillow + cv2) {min(ts):.1f} ms; "
